@@ -76,6 +76,23 @@ class GoBatch:
             mv[g, : len(m)] = m
         _l.check(self._lib, self._lib.elfb200_replay(self._ctx, mv.ctypes.data, stride, cnt.ctypes.data))
 
+    def place_handicap(self, stone_lists):
+        """GoState::applyHandicap for the batch in one launch: game g places the BLACK stones
+        ``stone_lists[g]`` (actions x*N+y) in order, each as PlaceHandicap does.  Only a game still at ply 1
+        takes stones; the ply stays 1 and white is to move once a stone is on the board.  Returns one bool
+        array per game: PlaceHandicap's verdict for each stone."""
+        assert len(stone_lists) == self.num_games
+        stride = max(1, max((len(s) for s in stone_lists), default=1))
+        st = np.zeros((self.num_games, stride), np.int16)
+        cnt = np.zeros(self.num_games, np.int32)
+        for g, s in enumerate(stone_lists):
+            cnt[g] = len(s)
+            st[g, : len(s)] = s
+        ok = np.zeros((self.num_games, stride), np.uint8)
+        _l.check(self._lib, self._lib.elfb200_place_handicap(self._ctx, st.ctypes.data, stride, cnt.ctypes.data,
+                                                             ok.ctypes.data))
+        return [ok[g, : cnt[g]].astype(bool) for g in range(self.num_games)]
+
     def synchronize(self):
         _l.check(self._lib, self._lib.elfb200_synchronize(self._ctx))
 

@@ -11,6 +11,11 @@ accept the values the engine was created with; ``final_score`` reports the value
 finished game (``getLastScore``), as the reference does.  Replies use the GTP wire format
 (``= text\\n\\n`` / ``? text\\n\\n``, optional numeric command id echoed).
 
+Beyond ``console_lib.py``, three GTP 2 commands start a handicap game: ``fixed_handicap n`` and
+``place_free_handicap n`` (2 <= n <= 9; both place the GTP fixed placement and reply with its vertices) and
+``set_free_handicap v1 v2 ...``.  They need an empty board and a board that can take handicap stones
+(``GoBatch.place_handicap``); afterwards white is to move.
+
 The reference console talks to its game thread by returning special actions from the
 ``human_actor`` callback; here the same special actions go straight into ``OnlineGame.human``.
 (The unmodified reference console can also be run against this engine through
@@ -19,6 +24,23 @@ The reference console talks to its game thread by returning special actions from
 import sys
 
 from . import online as _o
+
+HANDICAP_COMMANDS = ("fixed_handicap", "place_free_handicap", "set_free_handicap")
+
+
+def fixed_handicap_vertices(n, board_size):
+    """the GTP 2 fixed placement of ``n`` (2..9) handicap stones: 19x19 on the 4-4 points and their
+    midpoints (D4 Q16 D16 Q4, D10 Q10, K4 K16, K10), 9x9 by the same rule on the 3-3 points"""
+    lo = 3 if board_size >= 13 else 2
+    hi, mid = board_size - 1 - lo, board_size // 2
+    xy = [(lo, lo), (hi, hi), (lo, hi), (hi, lo)][: min(n, 4)]
+    if n >= 6:
+        xy += [(lo, mid), (hi, mid)]
+    if n >= 8:
+        xy += [(mid, lo), (mid, hi)]
+    if n >= 5 and n % 2 == 1:
+        xy.append((mid, mid))
+    return [_o.xy2move(x, y) for x, y in xy]
 
 
 class GtpConsole:
@@ -30,6 +52,9 @@ class GtpConsole:
         self.board_size = game.N
         self.exit = False
         self.commands = {k[3:]: getattr(self, k) for k in dir(self) if k.startswith("on_")}
+        if getattr(game.board, "place_handicap", None) is None:  # a board that cannot take handicap stones
+            for k in HANDICAP_COMMANDS:
+                del self.commands[k]
 
     # -- helpers ---------------------------------------------------------------------------------
     def check_player(self, player):  # console_lib.py:313-325
@@ -100,6 +125,42 @@ class GtpConsole:
 
     def on_showboard(self, items):
         return True, "\n" + self.game.showBoard().rstrip("\n")
+
+    # -- handicap (GTP 2 section 6.3.2) -----------------------------------------------------------
+    def _board_empty(self):
+        return int(self.game.info()[0]) == 1 and not self.game.board.stones()[0].any()
+
+    def on_fixed_handicap(self, items):
+        if not self._board_empty():
+            return False, "board not empty"
+        try:
+            n = int(items[1])
+        except (IndexError, ValueError):
+            n = 0
+        if not 2 <= n <= 9:
+            return False, "invalid number of stones"
+        vs = fixed_handicap_vertices(n, self.board_size)
+        if not self.game.place_handicap([_o.vertex2action(v, self.board_size) for v in vs]):
+            return False, "board not empty"
+        return True, " ".join(vs)
+
+    on_place_free_handicap = on_fixed_handicap  # the engine may choose any placement: the fixed one
+
+    def on_set_free_handicap(self, items):
+        if not self._board_empty():
+            return False, "board not empty"
+        acts = []
+        for v in items[1:]:
+            try:
+                a = _o.vertex2action(v, self.board_size)
+            except ValueError:  # off the board, or not a vertex
+                return False, "bad vertex list"
+            if a == self.board_size * self.board_size or a in acts:
+                return False, "bad vertex list"
+            acts.append(a)
+        if len(acts) < 2 or not self.game.place_handicap(acts):  # a stone the board refuses: nothing placed
+            return False, "bad vertex list"
+        return True, ""
 
     def on_final_score(self, items):
         s = self.game.getLastScore()

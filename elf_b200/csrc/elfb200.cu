@@ -230,6 +230,72 @@ __global__ void __launch_bounds__(BLOCK)
 }
 
 // ---------------------------------------------------------------------------------------
+// GoState::applyHandicap / PlaceHandicap (go_state.cc:62-71,130-132; board.cc:109-126) for all games in one
+// launch: game g places the BLACK stones stones[g][0 .. count[g]) in order.  Each stone is TryPlay for black,
+// whoever is to move (after the first stone white is, so the stored legal rows are not black's: black's
+// rows are computed here), then Play; afterwards the ply goes back to 1 and the last-move window to "none".
+// PlaceHandicap bypasses GoState::forward, so neither the superko record nor the history ring is written.
+// A game past ply 1 refuses every stone and is left as it is.  Games of one warp (9x9 packs three) may have
+// lists of different lengths: the warp runs to the longest, as in k_replay.
+template <int N>
+__global__ void __launch_bounds__(BLOCK)
+    k_place(DevState st, const int16_t* __restrict__ stones, int stride, const int32_t* __restrict__ count,
+            uint8_t* __restrict__ ok) {
+  __shared__ uint64_t s_zob[Geo<N>::ZOB];
+  load_zobrist<N>(s_zob);
+  const Lane L = make_lane<N>();
+  bool valid;
+  const int g = warp_game<N>(L, st.G, valid);
+  const int gs = valid ? g : 0;  // safe index for idle lanes (loads only)
+
+  const uint64_t rowv = valid ? st.cur[(size_t)gs * N + L.row] : 0ull;
+  uint32_t b = (uint32_t)rowv, w = (uint32_t)(rowv >> 32);
+  const uint64_t sav = valid ? st.sa[(size_t)gs * N + L.row] : 0ull;
+  uint32_t safe = (uint32_t)sav, atari = (uint32_t)(sav >> 32);
+  BoardMeta meta = load_meta(&st.meta[gs]);
+  uint64_t hash = st.hash[gs];
+  const bool open = valid && meta.ply <= 1;  // "the game has already started" (board.cc:111-112)
+  const int n = valid ? count[gs] : 0;
+  const int nmax = __reduce_max_sync(FULL, n);
+
+  for (int t = 0; t < nmax; ++t) {
+    const int a = t < n ? (int)stones[(size_t)gs * stride + t] : -1;
+    int pm = (open && a >= 0) ? (a % N) * N + (a / N) : MV_NONE;  // a = x*N + y  ->  p = y*N + x
+    {
+      // TryPlay(board, x, y, S_BLACK) (board.cc:788-827): empty, no simple-ko violation, not suicide
+      const bool ko_black = (meta.flags & F_KO_ACTIVE) && meta.ko_color == S_BLACK;
+      const uint32_t lb = legal_rows_cached<N>(b, w, safe, atari, L, ko_black, meta.ko_pt);
+      const int y = pm >= 0 ? pm / N : -1, x = pm >= 0 ? pm - y * N : 0;
+      const bool bit = (L.row == y) && ((lb >> x) & 1u);
+      const bool is_legal = game_any<N>(bit, L);
+      if (pm >= 0 && !is_legal) pm = MV_NONE;
+    }
+    if (pm >= 0) meta.next = S_BLACK;  // Play for ids->player == S_BLACK; leaves white to move
+    play_move_cached<N>(b, w, meta, hash, pm, s_zob, L, safe, atari);
+    if (pm >= 0) {
+      meta.ply = 1;  // board.cc:117-122
+      meta.last1 = meta.last2 = MV_INVALID;
+      if (L.row == 0) st.placed[(size_t)g * Geo<N>::P + pm] = 1;  // Info::last_placed = _ply (board.cc:1379)
+    }
+    if (ok && valid && L.row == 0 && t < n) ok[(size_t)g * stride + t] = pm >= 0 ? 1 : 0;
+  }
+
+  // legal rows for the side to move
+  const uint32_t own = meta.next == S_BLACK ? b : w, opp = meta.next == S_BLACK ? w : b;
+  const bool ko_applies = (meta.flags & F_KO_ACTIVE) && meta.ko_color == meta.next;
+  const uint32_t lnew = legal_rows_cached<N>(own, opp, safe, atari, L, ko_applies, meta.ko_pt);
+  if (open) {
+    st.cur[(size_t)g * N + L.row] = (uint64_t)b | ((uint64_t)w << 32);
+    st.sa[(size_t)g * N + L.row] = (uint64_t)safe | ((uint64_t)atari << 32);
+    st.legal[(size_t)g * N + L.row] = lnew;
+    if (L.row == 0) {
+      st.hash[g] = hash;
+      store_meta(&st.meta[g], meta);
+    }
+  }
+}
+
+// ---------------------------------------------------------------------------------------
 template <int N>
 __global__ void __launch_bounds__(BLOCK)
     k_export(DevState st, uint8_t* __restrict__ legal_out, uint8_t* __restrict__ stones_out,
@@ -831,15 +897,8 @@ int elfb200_step(elfb200_ctx* c, const int32_t* actions_host, uint8_t* ok_host) 
   return ELFB200_OK;
 }
 
-int elfb200_replay(elfb200_ctx* c, const int16_t* moves_host, int stride, const int32_t* count_host) {
-  if (!c || !moves_host || !count_host) return elfb200_fail(ELFB200_ERR_ARG, "NULL argument");
-  const int max_ply = c->N == 19 ? elfb200::Geo<19>::MAX_PLY : elfb200::Geo<9>::MAX_PLY;
-  if (stride <= 0 || stride > max_ply)
-    return elfb200_fail(ELFB200_ERR_ARG, "stride %d outside [1, %d]", stride, max_ply);
-  for (int g = 0; g < c->G; ++g)
-    if (count_host[g] < 0 || count_host[g] > stride)
-      return elfb200_fail(ELFB200_ERR_ARG, "count[%d] = %d outside [0, stride = %d]", g, count_host[g], stride);
-  CK(cudaSetDevice(c->device));
+// per-game action lists for k_replay / k_place: lists[G][stride] into d_replay (grown on demand), counts into d_actions
+static int upload_lists(elfb200_ctx* c, const int16_t* lists_host, int stride, const int32_t* count_host) {
   const size_t bytes = (size_t)c->G * (size_t)stride * sizeof(int16_t);
   if (bytes > c->d_replay_bytes) {
     if (c->d_replay) CK(cudaFree(c->d_replay));
@@ -850,11 +909,56 @@ int elfb200_replay(elfb200_ctx* c, const int16_t* moves_host, int stride, const 
   }
   memcpy(c->h_pin, count_host, (size_t)c->G * 4);
   CK(cudaMemcpyAsync(c->d_actions, c->h_pin, (size_t)c->G * 4, cudaMemcpyHostToDevice, c->stream));
-  CK(cudaMemcpyAsync(c->d_replay, moves_host, bytes, cudaMemcpyHostToDevice, c->stream));
+  CK(cudaMemcpyAsync(c->d_replay, lists_host, bytes, cudaMemcpyHostToDevice, c->stream));
+  return ELFB200_OK;
+}
+
+int elfb200_replay(elfb200_ctx* c, const int16_t* moves_host, int stride, const int32_t* count_host) {
+  if (!c || !moves_host || !count_host) return elfb200_fail(ELFB200_ERR_ARG, "NULL argument");
+  const int max_ply = c->N == 19 ? elfb200::Geo<19>::MAX_PLY : elfb200::Geo<9>::MAX_PLY;
+  if (stride <= 0 || stride > max_ply)
+    return elfb200_fail(ELFB200_ERR_ARG, "stride %d outside [1, %d]", stride, max_ply);
+  for (int g = 0; g < c->G; ++g)
+    if (count_host[g] < 0 || count_host[g] > stride)
+      return elfb200_fail(ELFB200_ERR_ARG, "count[%d] = %d outside [0, stride = %d]", g, count_host[g], stride);
+  CK(cudaSetDevice(c->device));
+  const int rc = upload_lists(c, moves_host, stride, count_host);
+  if (rc) return rc;
   DISPATCH_N(c, (k_replay<19><<<grid_for(c), BLOCK, 0, c->stream>>>(c->st, c->d_replay, stride, c->d_actions)),
              (k_replay<9><<<grid_for(c), BLOCK, 0, c->stream>>>(c->st, c->d_replay, stride, c->d_actions)));
   c->launches++;
   CK(cudaGetLastError());
+  CK(cudaStreamSynchronize(c->stream));
+  return ELFB200_OK;
+}
+
+int elfb200_place_handicap(elfb200_ctx* c, const int16_t* stones_host, int stride, const int32_t* count_host,
+                           uint8_t* ok_host) {
+  if (!c || !stones_host || !count_host) return elfb200_fail(ELFB200_ERR_ARG, "NULL argument");
+  const int P = c->N * c->N;
+  if (stride <= 0 || stride > P) return elfb200_fail(ELFB200_ERR_ARG, "stride %d outside [1, %d]", stride, P);
+  for (int g = 0; g < c->G; ++g) {
+    if (count_host[g] < 0 || count_host[g] > stride)
+      return elfb200_fail(ELFB200_ERR_ARG, "count[%d] = %d outside [0, stride = %d]", g, count_host[g], stride);
+    for (int t = 0; t < count_host[g]; ++t) {
+      const int a = stones_host[(size_t)g * stride + t];
+      if (a < 0 || a >= P)
+        return elfb200_fail(ELFB200_ERR_ARG, "stone %d of game %d: action %d outside [0, %d)", t, g, a, P);
+    }
+  }
+  CK(cudaSetDevice(c->device));
+  const int rc = upload_lists(c, stones_host, stride, count_host);
+  if (rc) return rc;
+  uint8_t* dok = nullptr;
+  if (ok_host) {  // G * stride <= G * (N*N + 1) bytes
+    dok = c->d_bytes;
+    CK(cudaMemsetAsync(dok, 0, (size_t)c->G * stride, c->stream));
+  }
+  DISPATCH_N(c, (k_place<19><<<grid_for(c), BLOCK, 0, c->stream>>>(c->st, c->d_replay, stride, c->d_actions, dok)),
+             (k_place<9><<<grid_for(c), BLOCK, 0, c->stream>>>(c->st, c->d_replay, stride, c->d_actions, dok)));
+  c->launches++;
+  CK(cudaGetLastError());
+  if (ok_host) CK(cudaMemcpyAsync(ok_host, dok, (size_t)c->G * stride, cudaMemcpyDeviceToHost, c->stream));
   CK(cudaStreamSynchronize(c->stream));
   return ELFB200_OK;
 }

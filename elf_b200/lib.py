@@ -36,6 +36,7 @@ SIGNATURES = {
     "elfb200_step": (ctypes.c_int, [vp, vp, vp]),
     "elfb200_step_dev": (ctypes.c_int, [vp, vp, vp]),
     "elfb200_replay": (ctypes.c_int, [vp, vp, ctypes.c_int, vp]),
+    "elfb200_place_handicap": (ctypes.c_int, [vp, vp, ctypes.c_int, vp, vp]),
     "elfb200_get_hash": (ctypes.c_int, [vp, vp]),
     "elfb200_get_info": (ctypes.c_int, [vp, vp]),
     "elfb200_get_stones": (ctypes.c_int, [vp, vp]),

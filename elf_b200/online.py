@@ -216,6 +216,22 @@ class OnlineGame:
         self._restart_game()
         return fv
 
+    # -- handicap -----------------------------------------------------------------------------------
+    def place_handicap(self, actions):
+        """GoState::applyHandicap on the game about to start: black stones at ``actions`` (x*N+y), each
+        placed as PlaceHandicap does (board.cc:109-126); afterwards white is to move and the ply is still 1.
+        Only on an empty board at ply 1.  If the board refuses any stone it is emptied again, so it never
+        holds part of a setup.  Returns True when all stones are on the board."""
+        i = self.info()
+        if int(i[0]) != 1 or self.board.stones()[0].any():
+            return False
+        ok = self.board.place_handicap([[int(a) for a in actions]])[0]
+        if not ok.all():
+            self.board.reset(None)
+            return False
+        self.search.reset(None)  # the tree's root is the empty board: it no longer matches (DESIGN 3 (ii))
+        return True
+
     # -- the human branch of act() ----------------------------------------------------------------
     def human(self, action):
         i = self.info()
@@ -228,6 +244,9 @@ class OnlineGame:
         if action == SA_CLEAR:
             if int(i[0]) != 1:  # !justStarted
                 self._finish_game("clear")
+            elif self.board.stones()[0].any():  # handicap stones, still ply 1: no game to finish
+                self.board.reset(None)
+                self.search.reset(None)
             return CLEARED
         if action == SA_RESIGN:
             self._finish_game("resign")

@@ -64,6 +64,12 @@ int elfb200_step_dev(elfb200_ctx* ctx, const int32_t* actions_dev, uint8_t* ok_d
  * pass).  A move GoState::forward refuses is skipped and the list goes on -- the reference ignores
  * forward()'s verdict there.  1 <= stride <= 2*N*N, 0 <= count[g] <= stride.  Synchronous. */
 int elfb200_replay(elfb200_ctx* ctx, const int16_t* moves_host, int stride, const int32_t* count_host);
+/* GoState::applyHandicap / PlaceHandicap (go_state.cc:62-71,130-132; board.cc:109-126) for every game in
+ * ONE launch: game g places BLACK stones stones_host[g*stride + 0 .. count_host[g]) in order (int16 actions
+ * x*N+y), each exactly as PlaceHandicap does.  ok_host uint8[G][stride] (may be NULL): PlaceHandicap's
+ * return value per stone.  1 <= stride <= N*N, 0 <= count[g] <= stride, actions in [0, N*N).  Synchronous. */
+int elfb200_place_handicap(elfb200_ctx* ctx, const int16_t* stones_host, int stride,
+                           const int32_t* count_host, uint8_t* ok_host);
 
 /* Board hash, GoState::getHashCode (go_state.h:170; set_color board.cc:38-51). uint64[G]. */
 int elfb200_get_hash(elfb200_ctx* ctx, uint64_t* hash_host);
