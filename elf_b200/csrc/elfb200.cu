@@ -4,6 +4,7 @@
 //   k_reset     clear selected games
 //   k_step      GoState::forward for a batch: validate, play, superko, next legal mask
 //   k_export    host-facing views (legal/stones/eyes by action index, info words, tt score)
+//   k_env_step  k_step + end of game (score, restart) + legal/info views: one ply of the device-resident env
 //   k_features  BoardFeature::extractAGZ, float32 [G][18][N][N]
 //   k_playout   whole random-policy games with the position (and the incremental safe/atari group
 //               masks) held in registers; to-terminal and steady-state ("stream") modes
@@ -28,13 +29,10 @@
 namespace elfb200 {
 
 // ---------------------------------------------------------------------------------------
+// GoState::reset of game g: the empty position, every point legal, no history, no superko record.
+// Each lane writes its own row (and row 0 the per-game words).
 template <int N>
-__global__ void __launch_bounds__(BLOCK) k_reset(DevState st, const uint8_t* __restrict__ mask) {
-  const Lane L = make_lane<N>();
-  bool valid;
-  const int g = warp_game<N>(L, st.G, valid);
-  if (!valid) return;
-  if (mask && !mask[g]) return;
+__device__ __forceinline__ void store_empty(const DevState& st, int g, const Lane& L) {
   st.cur[(size_t)g * N + L.row] = 0;
   st.sa[(size_t)g * N + L.row] = 0;
   st.legal[(size_t)g * N + L.row] = Geo<N>::ROWMASK;  // every point of the empty board is legal
@@ -47,19 +45,32 @@ __global__ void __launch_bounds__(BLOCK) k_reset(DevState st, const uint8_t* __r
   }
 }
 
-// ---------------------------------------------------------------------------------------
-// GoState::forward (go_state.cc:74-94) for all games.
 template <int N>
-__global__ void __launch_bounds__(BLOCK)
-    k_step(DevState st, const int32_t* __restrict__ actions, uint8_t* __restrict__ ok, unsigned* done_count,
-           volatile uint32_t* done_flag, uint32_t seq, uint8_t* ok_mapped) {
-  __shared__ uint64_t s_zob[Geo<N>::ZOB];
-  load_zobrist<N>(s_zob);
+__global__ void __launch_bounds__(BLOCK) k_reset(DevState st, const uint8_t* __restrict__ mask) {
   const Lane L = make_lane<N>();
   bool valid;
   const int g = warp_game<N>(L, st.G, valid);
-  const int gs = valid ? g : 0;  // safe index for idle lanes (loads only)
+  if (!valid) return;
+  if (mask && !mask[g]) return;
+  store_empty<N>(st, g, L);
+}
 
+// ---------------------------------------------------------------------------------------
+// GoState::forward (go_state.cc:74-94) of one game on its stored position, the body of k_step and
+// k_env_step: validate against the stored legal rows, play, superko scan and record, legal rows of the
+// new position.  The new position is left in `f` (store_position writes it); only the superko record is
+// written here.  Every lane of the warp calls it (warp collectives); idle lanes have valid = false.
+struct Forward {
+  uint32_t b, w, safe, atari;
+  BoardMeta meta;
+  uint64_t hash;
+  uint32_t lrow, lnew;  // legal rows before / after the move
+  int pm;               // the move played (p = y*N+x or MV_PASS), MV_NONE if refused or none
+};
+
+template <int N>
+__device__ __forceinline__ void forward_game(const DevState& st, const int32_t* __restrict__ actions, int g, int gs,
+                                             bool valid, const Lane& L, const uint64_t* s_zob, Forward& f) {
   uint64_t rowv = valid ? st.cur[(size_t)gs * N + L.row] : 0ull;
   uint32_t b = (uint32_t)rowv, w = (uint32_t)(rowv >> 32);
   // the incremental group status (safe / atari masks, board.cuh) is part of the stored position: a step
@@ -106,21 +117,48 @@ __global__ void __launch_bounds__(BLOCK)
   const uint32_t own = meta.next == S_BLACK ? b : w, opp = meta.next == S_BLACK ? w : b;
   const bool ko_applies = (meta.flags & F_KO_ACTIVE) && meta.ko_color == meta.next;
   const uint32_t lnew = legal_rows_cached<N>(own, opp, safe, atari, L, ko_applies, meta.ko_pt);
+  f.b = b;
+  f.w = w;
+  f.safe = safe;
+  f.atari = atari;
+  f.meta = meta;
+  f.hash = hash;
+  f.lrow = lrow;
+  f.lnew = lnew;
+  f.pm = pm;
+}
 
+// The position forward_game left in `f` becomes game g's stored position (called when a move was played).
+template <int N>
+__device__ __forceinline__ void store_position(const DevState& st, int g, const Lane& L, const Forward& f) {
+  const uint64_t nv = (uint64_t)f.b | ((uint64_t)f.w << 32);
+  st.cur[(size_t)g * N + L.row] = nv;
+  st.sa[(size_t)g * N + L.row] = (uint64_t)f.safe | ((uint64_t)f.atari << 32);
+  st.ring[((size_t)g * 8 + ((f.meta.ply - 2) & 7)) * N + L.row] = nv;  // go_state.cc:90-92
+  st.legal[(size_t)g * N + L.row] = f.lnew;
+  if (L.row == 0) {
+    st.hash[g] = f.hash;
+    store_meta(&st.meta[g], f.meta);
+    if (f.pm >= 0) st.placed[(size_t)g * Geo<N>::P + f.pm] = (uint16_t)(f.meta.ply - 1);  // Info::last_placed = _ply (board.cc:680,1379)
+  }
+}
+
+// GoState::forward (go_state.cc:74-94) for all games.
+template <int N>
+__global__ void __launch_bounds__(BLOCK)
+    k_step(DevState st, const int32_t* __restrict__ actions, uint8_t* __restrict__ ok, unsigned* done_count,
+           volatile uint32_t* done_flag, uint32_t seq, uint8_t* ok_mapped) {
+  __shared__ uint64_t s_zob[Geo<N>::ZOB];
+  load_zobrist<N>(s_zob);
+  const Lane L = make_lane<N>();
+  bool valid;
+  const int g = warp_game<N>(L, st.G, valid);
+  const int gs = valid ? g : 0;  // safe index for idle lanes (loads only)
+  Forward f;
+  forward_game<N>(st, actions, g, gs, valid, L, s_zob, f);
   if (valid) {
-    if (pm != MV_NONE) {
-      const uint64_t nv = (uint64_t)b | ((uint64_t)w << 32);
-      st.cur[(size_t)g * N + L.row] = nv;
-      st.sa[(size_t)g * N + L.row] = (uint64_t)safe | ((uint64_t)atari << 32);
-      st.ring[((size_t)g * 8 + ((meta.ply - 2) & 7)) * N + L.row] = nv;  // go_state.cc:90-92
-      st.legal[(size_t)g * N + L.row] = lnew;
-      if (L.row == 0) {
-        st.hash[g] = hash;
-        store_meta(&st.meta[g], meta);
-        if (pm >= 0) st.placed[(size_t)g * Geo<N>::P + pm] = (uint16_t)(meta.ply - 1);  // Info::last_placed = _ply (board.cc:680,1379)
-      }
-    }
-    if (ok && L.row == 0) ok[g] = pm != MV_NONE ? 1 : 0;
+    if (f.pm != MV_NONE) store_position<N>(st, g, L, f);
+    if (ok && L.row == 0) ok[g] = f.pm != MV_NONE ? 1 : 0;
   }
   // host-driven step (elfb200_step): the last CTA to finish copies the accept flags to the mapped host window
   // in 16-byte pieces (4096 one-byte PCIe writes from as many warps measured ~14 us) and raises the completion
@@ -296,6 +334,37 @@ __global__ void __launch_bounds__(BLOCK)
 }
 
 // ---------------------------------------------------------------------------------------
+// Host-facing views of one game, shared by k_export and k_env_step.
+// legal uint8[G][N*N+1] by action index (elfb200_get_legal): this lane's legal row `l`, pass always legal.
+template <int N>
+__device__ __forceinline__ void write_legal(uint8_t* __restrict__ legal_out, int g, const Lane& L, uint32_t l) {
+  constexpr int P = Geo<N>::P;
+  for (int x = 0; x < N; ++x) legal_out[(size_t)g * (P + 1) + x * N + L.row] = (l >> x) & 1u;
+  if (L.row == 0) legal_out[(size_t)g * (P + 1) + P] = 1;
+}
+
+// info int32[ELFB200_INFO_FIELDS] of one game (elfb200_get_info)
+template <int N>
+__device__ __forceinline__ void write_info(int32_t* __restrict__ o, const BoardMeta& meta) {
+  auto p2a = [](int p) -> int {
+    if (p == MV_PASS) return Geo<N>::P;
+    if (p < 0) return -1;
+    return (p % N) * N + p / N;
+  };
+  o[0] = meta.ply;
+  o[1] = meta.next;
+  o[2] = meta.b_cap;
+  o[3] = meta.w_cap;
+  o[4] = p2a(meta.last1);
+  o[5] = p2a(meta.last2);
+  o[6] = (meta.flags & F_KO_ACTIVE) ? p2a(meta.ko_pt) : -1;
+  o[7] = meta.ko_color;
+  o[8] = 0;
+  o[9] = is_terminated<N>(meta) ? 1 : 0;
+  o[10] = (meta.last1 == MV_PASS && meta.last2 == MV_PASS) ? 1 : 0;
+  o[11] = (meta.flags & F_SUPERKO) ? 1 : 0;
+}
+
 template <int N>
 __global__ void __launch_bounds__(BLOCK)
     k_export(DevState st, uint8_t* __restrict__ legal_out, uint8_t* __restrict__ stones_out,
@@ -309,11 +378,7 @@ __global__ void __launch_bounds__(BLOCK)
   const uint32_t b = (uint32_t)rowv, w = (uint32_t)(rowv >> 32);
   const BoardMeta meta = load_meta(&st.meta[gs]);
   constexpr int P = Geo<N>::P;
-  if (legal_out && valid) {
-    const uint32_t l = st.legal[(size_t)g * N + L.row];
-    for (int x = 0; x < N; ++x) legal_out[(size_t)g * (P + 1) + x * N + L.row] = (l >> x) & 1u;
-    if (L.row == 0) legal_out[(size_t)g * (P + 1) + P] = 1;
-  }
+  if (legal_out && valid) write_legal<N>(legal_out, g, L, st.legal[(size_t)g * N + L.row]);
   if (stones_out && valid) {
     for (int x = 0; x < N; ++x)
       stones_out[(size_t)g * P + x * N + L.row] = ((b >> x) & 1u) | (((w >> x) & 1u) << 1);
@@ -329,25 +394,48 @@ __global__ void __launch_bounds__(BLOCK)
     const int sc = tt_score<N>(b, w, L);
     if (valid && L.row == 0) score_out[g] = sc;
   }
-  if (info_out && valid && L.row == 0) {
-    auto p2a = [](int p) -> int {
-      if (p == MV_PASS) return Geo<N>::P;
-      if (p < 0) return -1;
-      return (p % N) * N + p / N;
-    };
-    int32_t* o = info_out + (size_t)g * ELFB200_INFO_FIELDS;
-    o[0] = meta.ply;
-    o[1] = meta.next;
-    o[2] = meta.b_cap;
-    o[3] = meta.w_cap;
-    o[4] = p2a(meta.last1);
-    o[5] = p2a(meta.last2);
-    o[6] = (meta.flags & F_KO_ACTIVE) ? p2a(meta.ko_pt) : -1;
-    o[7] = meta.ko_color;
-    o[8] = 0;
-    o[9] = is_terminated<N>(meta) ? 1 : 0;
-    o[10] = (meta.last1 == MV_PASS && meta.last2 == MV_PASS) ? 1 : 0;
-    o[11] = (meta.flags & F_SUPERKO) ? 1 : 0;
+  if (info_out && valid && L.row == 0) write_info<N>(info_out + (size_t)g * ELFB200_INFO_FIELDS, meta);
+}
+
+// ---------------------------------------------------------------------------------------
+// One ply of the device-resident environment (elfb200_env_step): GoState::forward of every game as k_step
+// does, then every game that has ended (GoState::terminated: two passes, positional superko or the 2N^2
+// ply cap; also a game stepped to its end through the other entry points, whatever its action) is scored
+// with GoState::evaluate(komi) and restarted from the empty position as k_reset does.  legal / info
+// describe the position now stored.  Each output may be NULL.
+template <int N>
+__global__ void __launch_bounds__(BLOCK)
+    k_env_step(DevState st, const int32_t* __restrict__ actions, float komi, uint8_t* __restrict__ ok,
+               uint8_t* __restrict__ done_out, float* __restrict__ value, uint8_t* __restrict__ legal_out,
+               int32_t* __restrict__ info_out) {
+  __shared__ uint64_t s_zob[Geo<N>::ZOB];
+  load_zobrist<N>(s_zob);
+  const Lane L = make_lane<N>();
+  bool valid;
+  const int g = warp_game<N>(L, st.G, valid);
+  const int gs = valid ? g : 0;  // safe index for idle lanes (loads only)
+  Forward f;
+  forward_game<N>(st, actions, g, gs, valid, L, s_zob, f);
+
+  // GoState::evaluate (go_state.h:194-203) in elfb200_evaluate's float arithmetic, black's point of view.
+  // tt_score is a warp collective: it runs when any game of the warp has ended, on every lane.
+  const bool done = valid && is_terminated<N>(f.meta);
+  float v = 0.f;
+  if (__any_sync(FULL, done)) {
+    const int sc = tt_score<N>(f.b, f.w, L);
+    if (done) v = (f.meta.flags & F_SUPERKO) ? (f.meta.next == S_BLACK ? 1.0f : -1.0f) : (float)sc - komi;
+  }
+  if (!valid) return;
+  if (done)
+    store_empty<N>(st, g, L);
+  else if (f.pm != MV_NONE)
+    store_position<N>(st, g, L, f);
+  if (legal_out) write_legal<N>(legal_out, g, L, done ? Geo<N>::ROWMASK : f.pm != MV_NONE ? f.lnew : f.lrow);
+  if (L.row == 0) {
+    if (info_out) write_info<N>(info_out + (size_t)g * ELFB200_INFO_FIELDS, done ? initial_meta() : f.meta);
+    if (ok) ok[g] = f.pm != MV_NONE ? 1 : 0;
+    if (done_out) done_out[g] = done ? 1 : 0;
+    if (value) value[g] = v;
   }
 }
 
@@ -860,6 +948,30 @@ int elfb200_step_dev(elfb200_ctx* c, const int32_t* actions_dev, uint8_t* ok_dev
   return ELFB200_OK;
 }
 
+int elfb200_env_step(elfb200_ctx* c, const int32_t* actions_dev, float komi, uint8_t* ok_dev, uint8_t* done_dev,
+                     float* value_dev, uint8_t* legal_dev, int32_t* info_dev) {
+  if (!c || !actions_dev) return elfb200_fail(ELFB200_ERR_ARG, "ctx/actions is NULL");
+  CK(cudaSetDevice(c->device));
+  DISPATCH_N(c,
+             (k_env_step<19><<<grid_for(c), BLOCK, 0, c->stream>>>(c->st, actions_dev, komi, ok_dev, done_dev, value_dev,
+                                                                   legal_dev, info_dev)),
+             (k_env_step<9><<<grid_for(c), BLOCK, 0, c->stream>>>(c->st, actions_dev, komi, ok_dev, done_dev, value_dev,
+                                                                  legal_dev, info_dev)));
+  c->launches++;
+  CK(cudaGetLastError());
+  return ELFB200_OK;
+}
+
+int elfb200_reset_dev(elfb200_ctx* c, const uint8_t* mask_dev) {
+  if (!c) return elfb200_fail(ELFB200_ERR_ARG, "ctx is NULL");
+  CK(cudaSetDevice(c->device));
+  DISPATCH_N(c, (k_reset<19><<<grid_for(c), BLOCK, 0, c->stream>>>(c->st, mask_dev)),
+             (k_reset<9><<<grid_for(c), BLOCK, 0, c->stream>>>(c->st, mask_dev)));
+  c->launches++;
+  CK(cudaGetLastError());
+  return ELFB200_OK;
+}
+
 int elfb200_step(elfb200_ctx* c, const int32_t* actions_host, uint8_t* ok_host) {
   if (!c || !actions_host) return elfb200_fail(ELFB200_ERR_ARG, "ctx/actions is NULL");
   CK(cudaSetDevice(c->device));
@@ -992,6 +1104,12 @@ int elfb200_get_info(elfb200_ctx* c, int32_t* info_host) {
                      cudaMemcpyDeviceToHost, c->stream));
   CK(cudaStreamSynchronize(c->stream));
   return ELFB200_OK;
+}
+
+int elfb200_observe_dev(elfb200_ctx* c, uint8_t* legal_dev, int32_t* info_dev) {
+  if (!c) return elfb200_fail(ELFB200_ERR_ARG, "ctx is NULL");
+  CK(cudaSetDevice(c->device));
+  return run_export(c, legal_dev, nullptr, nullptr, 0, info_dev, nullptr);
 }
 
 int elfb200_get_stones(elfb200_ctx* c, uint8_t* stones_host) {

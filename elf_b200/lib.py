@@ -35,6 +35,9 @@ SIGNATURES = {
     "elfb200_reset": (ctypes.c_int, [vp, vp]),
     "elfb200_step": (ctypes.c_int, [vp, vp, vp]),
     "elfb200_step_dev": (ctypes.c_int, [vp, vp, vp]),
+    "elfb200_env_step": (ctypes.c_int, [vp, vp, ctypes.c_float, vp, vp, vp, vp, vp]),
+    "elfb200_reset_dev": (ctypes.c_int, [vp, vp]),
+    "elfb200_observe_dev": (ctypes.c_int, [vp, vp, vp]),
     "elfb200_replay": (ctypes.c_int, [vp, vp, ctypes.c_int, vp]),
     "elfb200_place_handicap": (ctypes.c_int, [vp, vp, ctypes.c_int, vp, vp]),
     "elfb200_get_hash": (ctypes.c_int, [vp, vp]),

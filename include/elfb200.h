@@ -58,6 +58,22 @@ int elfb200_reset(elfb200_ctx* ctx, const uint8_t* mask_host);
 int elfb200_step(elfb200_ctx* ctx, const int32_t* actions_host, uint8_t* ok_host);
 /* Same with device buffers, asynchronous on the context stream. */
 int elfb200_step_dev(elfb200_ctx* ctx, const int32_t* actions_dev, uint8_t* ok_dev);
+/* One ply of a device-resident environment, asynchronous on the context stream, no host copies and no
+ * synchronisation (capturable in a CUDA graph on elfb200_stream).  GoState::forward(actions[g]) for
+ * every game (actions < 0: untouched), then for every game that has ended (GoState::terminated: two
+ * passes, positional superko or the 2*N*N ply cap, also a game that had ended before the call):
+ * done[g] = 1, value[g] = GoState::evaluate(komi) (black's view; go_state.h:194-203; 0 where not done)
+ * and the game is restarted (GoState::reset).  ok[g] is forward's verdict.  legal uint8[G][N*N+1] /
+ * info int32[G][12] describe the positions now to move, as elfb200_get_legal / elfb200_get_info.
+ * Every output is a device pointer and may be NULL. */
+int elfb200_env_step(elfb200_ctx* ctx, const int32_t* actions_dev, float komi, uint8_t* ok_dev,
+                     uint8_t* done_dev, float* value_dev, uint8_t* legal_dev, int32_t* info_dev);
+/* GoState::reset for games with mask_dev[g] != 0 (all games if mask_dev == NULL), asynchronous on the
+ * context stream. */
+int elfb200_reset_dev(elfb200_ctx* ctx, const uint8_t* mask_dev);
+/* legal / info of the stored positions into device buffers (each may be NULL), asynchronous: the first
+ * observation after elfb200_reset or elfb200_place_handicap. */
+int elfb200_observe_dev(elfb200_ctx* ctx, uint8_t* legal_dev, int32_t* info_dev);
 /* GoStateExtOffline::switchBeforeMove (common/go_state_ext.h:305-312), the replay step of the
  * training loop (train/game_train.cc:22-45), for every game in ONE launch: game g is reset and
  * moves_host[g*stride + 0 .. count_host[g]) are forwarded in order (int16 actions x*N+y, N*N =
@@ -148,7 +164,8 @@ int elfb200_playout_stream_launch(elfb200_ctx* ctx, uint64_t seed, uint64_t firs
  * 1.35 vs 1.00 G at 12,288), one row per lane below.  Same results either way. */
 int elfb200_set_playout_layout(elfb200_ctx* ctx, int layout);
 
-/* Number of kernels this library has launched since creation (bench gpu_launches). */
+/* Number of kernels this library has launched since creation (bench gpu_launches).  Counts enqueues by
+ * the calls above; replays of a CUDA graph that captured them are not counted. */
 int64_t elfb200_launch_count(const elfb200_ctx* ctx);
 
 #ifdef __cplusplus
