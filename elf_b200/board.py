@@ -93,6 +93,46 @@ class GoBatch:
                                                              ok.ctypes.data))
         return [ok[g, : cnt[g]].astype(bool) for g in range(self.num_games)]
 
+    # -- GoState's copy constructor -----------------------------------------------------------
+    def gather(self, src, index):
+        """copy games from the batch ``src`` (same board size and device, not this batch): game i becomes a
+        copy of src's game ``index[i]`` for ``index[i]`` in [0, src.num_games); any other value leaves game
+        i as it is.  ``index``: G entries, a list / numpy array (synchronous), or an int32 CUDA tensor on
+        this batch's device (asynchronous: ordered after the caller's current stream and before its next
+        work, with events only, so it can be captured in a CUDA graph).  A search handle on this batch keeps
+        its trees: reset the copied games' trees before their next search."""
+        if getattr(index, "is_cuda", False):
+            return self._gather_dev(src, index)
+        a = np.asarray(index)
+        if a.dtype != np.int32:  # out-of-range values stay out of range (untouched games) in int32
+            a = np.clip(a, -1, src.num_games)
+        a = np.ascontiguousarray(a, dtype=np.int32)
+        assert a.shape == (self.num_games,)
+        _l.check(self._lib, self._lib.elfb200_gather_games(self._ctx, src._ctx, a.ctypes.data))
+
+    def _gather_dev(self, src, index):
+        import torch
+
+        dev = torch.device("cuda", self.device)
+        if index.dtype != torch.int32 or tuple(index.shape) != (self.num_games,) or not index.is_contiguous() \
+                or index.device != dev:
+            raise ValueError(f"index must be a contiguous int32 tensor of shape ({self.num_games},) on {dev}")
+        if getattr(self, "_gather_ev", None) is None:
+            self._gather_ev = [torch.cuda.Event() for _ in range(3)]
+            self._gather_stream = torch.cuda.ExternalStream(self.stream, device=dev)
+        ev, s_dst = self._gather_ev, self._gather_stream
+        s_src = torch.cuda.ExternalStream(src.stream, device=dev)
+        cur = torch.cuda.current_stream(dev)
+        # both context streams join the caller's stream before the copy and rejoin it afterwards
+        ev[0].record(cur)
+        s_dst.wait_event(ev[0])
+        s_src.wait_event(ev[0])
+        _l.check(self._lib, self._lib.elfb200_gather_games_dev(self._ctx, src._ctx, index.data_ptr()))
+        ev[1].record(s_dst)
+        cur.wait_event(ev[1])
+        ev[2].record(s_src)
+        cur.wait_event(ev[2])
+
     def synchronize(self):
         _l.check(self._lib, self._lib.elfb200_synchronize(self._ctx))
 

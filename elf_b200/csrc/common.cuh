@@ -385,6 +385,8 @@ struct elfb200_ctx {
   size_t map_ok_off = 0, map_flag_off = 0;  // byte offsets of the accept flags / completion flag in the mapped window
   uint32_t step_seq = 0;        // sequence number the last CTA writes into the mapped completion flag
   int64_t launches = 0;
+  // fork / join of elfb200_gather_games_dev with this context as the destination (cudaEventDisableTiming)
+  cudaEvent_t ev_gather[2] = {nullptr, nullptr};
   // move lists of elfb200_replay (grown on demand)
   int16_t* d_replay = nullptr;
   size_t d_replay_bytes = 0;

@@ -8,6 +8,7 @@
 //   k_features  BoardFeature::extractAGZ, float32 [G][18][N][N]
 //   k_playout   whole random-policy games with the position (and the incremental safe/atari group
 //               masks) held in registers; to-terminal and steady-state ("stream") modes
+//   k_gather    copy games from another batch (GoState's copy constructor); no geometry, one kernel for both sizes
 //
 // HBM layout (structure of arrays, G games):
 //   cur   uint64 [G][N]      current position, row y = black_row | white_row << 32
@@ -793,6 +794,52 @@ __global__ void __launch_bounds__(PLAYOUT_WARPS * 32)
   }
 }
 
+// ---------------------------------------------------------------------------------------
+// GoState's copy constructor (go_state.h:117-124, copyBoard board.cc:128-132) from one batch into another:
+// dst game i := src game index[i] for index[i] in [0, src.G); any other value leaves game i as it is.  A
+// game's stored state is its DevState blocks and nothing else, so the copy needs no board geometry and one
+// kernel serves both board sizes: one warp per destination game, the lanes striding over each per-game
+// block in the widest word its alignment allows (16 B for the history ring and the superko record, whose
+// per-game blocks are multiples of 16 B; 8 / 4 / 2 B for the rows and `placed`).  Of the superko record only
+// sk[0 .. sk_n) is copied: every reader (superko_scan in k_step / k_env_step / k_replay, the search's tree
+// descent) stops at sk_n and every writer appends at sk_n.
+constexpr int GATHER_THREADS = 256;
+
+__global__ void __launch_bounds__(GATHER_THREADS)
+    k_gather(DevState dst, DevState src, const int32_t* __restrict__ index, int N) {
+  const int lane = threadIdx.x & 31;
+  const int gd = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+  if (gd >= dst.G) return;
+  const int gs = index[gd];
+  if (gs < 0 || gs >= src.G) return;
+  const size_t d = (size_t)gd, s = (size_t)gs;
+  const int P = N * N, max_ply = 2 * P;
+  {  // history ring: 8 N rows = 4 N 16-byte words
+    const uint4* a = reinterpret_cast<const uint4*>(src.ring + s * 8 * N);
+    uint4* b = reinterpret_cast<uint4*>(dst.ring + d * 8 * N);
+    for (int i = lane; i < 4 * N; i += 32) b[i] = __ldg(a + i);
+  }
+  const int nsk = min(max(__ldg(src.sk_n + s), 0), max_ply);
+  {  // superko record: the pairs of sk[0 .. nsk), then an odd last entry
+    const uint64_t* a = src.sk + s * max_ply;
+    uint64_t* b = dst.sk + d * max_ply;
+    for (int i = lane; i < nsk / 2; i += 32) reinterpret_cast<uint4*>(b)[i] = __ldg(reinterpret_cast<const uint4*>(a) + i);
+    if ((nsk & 1) && lane == 0) b[nsk - 1] = __ldg(a + nsk - 1);
+  }
+  for (int i = lane; i < N; i += 32) {  // rows: position, group status, legal moves
+    dst.cur[d * N + i] = __ldg(src.cur + s * N + i);
+    dst.sa[d * N + i] = __ldg(src.sa + s * N + i);
+    dst.legal[d * N + i] = __ldg(src.legal + s * N + i);
+  }
+  for (int i = lane; i < P; i += 32) dst.placed[d * P + i] = __ldg(src.placed + s * P + i);
+  if (lane == 0) {
+    dst.hash[d] = __ldg(src.hash + s);
+    dst.sk_n[d] = nsk;
+  } else if (lane == 1) {
+    store_meta(&dst.meta[d], load_meta(&src.meta[s]));
+  }
+}
+
 }  // namespace elfb200
 
 // =========================================================================================
@@ -844,6 +891,9 @@ int elfb200_create(int board_size, int num_games, int device, elfb200_ctx** out)
   auto build = [&]() -> int {
   const size_t N = board_size, G = num_games, P = N * N, MAXPLY = 2 * P;
   CK(cudaStreamCreateWithFlags(&c->stream, cudaStreamNonBlocking));
+#if !defined(ELFB200_SIMT_EMU)  // the emulator build orders nothing (stream_after)
+  for (cudaEvent_t& e : c->ev_gather) CK(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
+#endif
   CK(cudaMalloc(&c->st.cur, G * N * 8));
   CK(cudaMalloc(&c->st.ring, G * 8 * N * 8));
   CK(cudaMalloc(&c->st.legal, G * N * 4));
@@ -906,6 +956,8 @@ void elfb200_destroy(elfb200_ctx* c) {
     if (p) cudaFree(p);
   if (c->h_pin) cudaFreeHost(c->h_pin);
   if (c->h_map) cudaFreeHost(c->h_map);
+  for (cudaEvent_t e : c->ev_gather)
+    if (e) cudaEventDestroy(e);
   if (c->stream) cudaStreamDestroy(c->stream);
   delete c;
 }
@@ -1072,6 +1124,58 @@ int elfb200_place_handicap(elfb200_ctx* c, const int16_t* stones_host, int strid
   CK(cudaGetLastError());
   if (ok_host) CK(cudaMemcpyAsync(ok_host, dok, (size_t)c->G * stride, cudaMemcpyDeviceToHost, c->stream));
   CK(cudaStreamSynchronize(c->stream));
+  return ELFB200_OK;
+}
+
+static int check_gather(const elfb200_ctx* dst, const elfb200_ctx* src, const int32_t* index) {
+  if (!dst || !src || !index) return elfb200_fail(ELFB200_ERR_ARG, "dst/src/index is NULL");
+  if (dst == src) return elfb200_fail(ELFB200_ERR_ARG, "dst and src are the same context (an in-place permutation would race)");
+  if (dst->N != src->N) return elfb200_fail(ELFB200_ERR_ARG, "board sizes differ (dst %d, src %d)", dst->N, src->N);
+  if (dst->device != src->device)
+    return elfb200_fail(ELFB200_ERR_ARG, "devices differ (dst %d, src %d)", dst->device, src->device);
+  return ELFB200_OK;
+}
+
+// `waiter`'s later work runs after the work already on `first` (event `ev`).  The SIMT emulator build runs all
+// work in issue order, so there it has nothing to order.
+static int stream_after(cudaStream_t waiter, cudaStream_t first, cudaEvent_t ev) {
+#if defined(ELFB200_SIMT_EMU)
+  (void)waiter, (void)first, (void)ev;
+#else
+  CK(cudaEventRecord(ev, first));
+  CK(cudaStreamWaitEvent(waiter, ev, 0));
+#endif
+  return ELFB200_OK;
+}
+
+// k_gather on dst's stream, after the work already on src's stream (fork); src's later work waits for the
+// copy (join), so it cannot change a game while the game is read
+static int gather_launch(elfb200_ctx* dst, const elfb200_ctx* src, const int32_t* index_dev) {
+  int rc = stream_after(dst->stream, src->stream, dst->ev_gather[0]);
+  if (rc) return rc;
+  const int grid = (int)(((size_t)dst->G * 32 + GATHER_THREADS - 1) / GATHER_THREADS);
+  k_gather<<<grid, GATHER_THREADS, 0, dst->stream>>>(dst->st, src->st, index_dev, dst->N);
+  dst->launches++;
+  CK(cudaGetLastError());
+  return stream_after(src->stream, dst->stream, dst->ev_gather[1]);
+}
+
+int elfb200_gather_games_dev(elfb200_ctx* dst, const elfb200_ctx* src, const int32_t* index_dev) {
+  int rc = check_gather(dst, src, index_dev);
+  if (rc) return rc;
+  CK(cudaSetDevice(dst->device));
+  return gather_launch(dst, src, index_dev);
+}
+
+int elfb200_gather_games(elfb200_ctx* dst, const elfb200_ctx* src, const int32_t* index_host) {
+  int rc = check_gather(dst, src, index_host);
+  if (rc) return rc;
+  CK(cudaSetDevice(dst->device));
+  memcpy(dst->h_pin, index_host, (size_t)dst->G * 4);
+  CK(cudaMemcpyAsync(dst->d_actions, dst->h_pin, (size_t)dst->G * 4, cudaMemcpyHostToDevice, dst->stream));
+  rc = gather_launch(dst, src, dst->d_actions);
+  if (rc) return rc;
+  CK(cudaStreamSynchronize(dst->stream));
   return ELFB200_OK;
 }
 

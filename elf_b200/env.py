@@ -151,6 +151,21 @@ class GoEnv:
 
         return self._enqueue(call, d4)
 
+    def load(self, src, index, d4=None):
+        """copy positions into this env's games: game i becomes a copy of game ``index[i]`` of ``src`` (a
+        :class:`GoBatch` or a ``GoEnv`` of the same board size on the same device) for ``index[i]`` in
+        [0, src.num_games); any other value leaves game i as it is.  ``index``: int32 [G] on the env's device,
+        e.g. ``torch.where(done, pick, -1)`` to restart finished games from a pool of positions.  ``ok``,
+        ``done`` and ``value`` of the loaded games are cleared, as ``reset`` clears them.  Returns the
+        observation of every game, as ``observe``."""
+        board = src.board if isinstance(src, GoEnv) else src
+        self._check(index, (torch.int32,), (self.num_games,), "index")
+        loaded = (index >= 0) & (index < board.num_games)
+        for t in (self.ok, self.done, self.value):
+            t.masked_fill_(loaded, 0)
+        self.board.gather(board, index if self._cuda else index.numpy())
+        return self.observe(d4)
+
     def observe(self, d4=None):
         """the observation of the stored positions without playing, e.g. after ``board.place_handicap``"""
         L, c = self._lib, self._ctx

@@ -40,6 +40,8 @@ SIGNATURES = {
     "elfb200_observe_dev": (ctypes.c_int, [vp, vp, vp]),
     "elfb200_replay": (ctypes.c_int, [vp, vp, ctypes.c_int, vp]),
     "elfb200_place_handicap": (ctypes.c_int, [vp, vp, ctypes.c_int, vp, vp]),
+    "elfb200_gather_games": (ctypes.c_int, [vp, vp, vp]),
+    "elfb200_gather_games_dev": (ctypes.c_int, [vp, vp, vp]),
     "elfb200_get_hash": (ctypes.c_int, [vp, vp]),
     "elfb200_get_info": (ctypes.c_int, [vp, vp]),
     "elfb200_get_stones": (ctypes.c_int, [vp, vp]),

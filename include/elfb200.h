@@ -86,6 +86,14 @@ int elfb200_replay(elfb200_ctx* ctx, const int16_t* moves_host, int stride, cons
  * return value per stone.  1 <= stride <= N*N, 0 <= count[g] <= stride, actions in [0, N*N).  Synchronous. */
 int elfb200_place_handicap(elfb200_ctx* ctx, const int16_t* stones_host, int stride,
                            const int32_t* count_host, uint8_t* ok_host);
+/* GoState's copy constructor (go_state.h:117-124; copyBoard board.cc:128-132) from one batch into another:
+ * dst game i := src game index[i] for index[i] in [0, G_src); other values leave game i untouched.
+ * index has G_dst entries.  Same board size and device; dst != src.  The _dev form is asynchronous on dst's
+ * stream and orders itself after the work already on src's stream, and src's later work after itself;
+ * capturable when both streams are part of the capture.  The host form is synchronous.  A search handle on
+ * dst keeps its trees: reset the copied games' trees (elfb200_mcts_reset) before their next search. */
+int elfb200_gather_games(elfb200_ctx* dst, const elfb200_ctx* src, const int32_t* index_host);
+int elfb200_gather_games_dev(elfb200_ctx* dst, const elfb200_ctx* src, const int32_t* index_dev);
 
 /* Board hash, GoState::getHashCode (go_state.h:170; set_color board.cc:38-51). uint64[G]. */
 int elfb200_get_hash(elfb200_ctx* ctx, uint64_t* hash_host);
