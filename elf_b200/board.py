@@ -22,6 +22,16 @@ class GoBatch:
         self.device = device
         self._children = []  # weakrefs to objects holding handles into this context (MctsBatch)
 
+    def new_like(self, num_games):
+        """a new batch of ``num_games`` empty games of this batch's board size, on its device and library"""
+        gb = GoBatch.__new__(GoBatch)
+        gb._lib = self._lib
+        gb._ctx = _l.vp()
+        _l.check(gb._lib, gb._lib.elfb200_create(self.board_size, num_games, self.device, ctypes.byref(gb._ctx)))
+        gb.num_games, gb.board_size, gb.num_actions, gb.device = num_games, self.board_size, self.num_actions, self.device
+        gb._children = []
+        return gb
+
     def close(self):
         if getattr(self, "_ctx", None):
             for w in getattr(self, "_children", []):
@@ -279,6 +289,73 @@ class GoBatch:
 
     def playout_stream_launch(self, seed, first_game_id=0, plies_per_slot=512):
         _l.check(self._lib, self._lib.elfb200_playout_stream_launch(self._ctx, seed, first_game_id, plies_per_slot))
+
+    # -- ownership and dead stones -------------------------------------------------------------
+    def ownership(self, playouts, seed=0, max_plies=None, out=None, trace=False):
+        """Monte-Carlo ownership: ``playouts`` (K) random playouts (the policy of
+        include/elfb200_playout_policy.h, draw id g*K + k) from every stored position, which stays as it is.
+        Returns int32 ``[G, 2, N*N]`` by action x*N+y: how many playouts end with the point in black's [0] /
+        white's [1] area (simple_tt_scoring's view).  A game that ended by two passes is played on; one that
+        ended by superko or the ply cap is counted as it stands.  ``trace=True`` also returns the final hash
+        (uint64) and plies (int32) of every playout, ``[G, K]`` each.  With ``out``, a contiguous int32 CUDA
+        tensor of shape ``[G, 2, N*N]`` on this batch's device, the counts are written there asynchronously,
+        ordered after the caller's current stream and before its next work with events only (capturable in a
+        CUDA graph after one call of either form has set up the scratch); ``out`` is returned."""
+        n, G, K = self.board_size, self.num_games, int(playouts)
+        max_plies = 2 * n * n if max_plies is None else int(max_plies)
+        seed = int(seed) & 0xFFFFFFFFFFFFFFFF
+        if out is not None:
+            return self._ownership_dev(K, seed, max_plies, out)
+        counts = np.empty((G, 2, n * n), np.int32)
+        fh = np.empty((G, K), np.uint64) if trace else None
+        pl = np.empty((G, K), np.int32) if trace else None
+        _l.check(self._lib, self._lib.elfb200_ownership(
+            self._ctx, K, seed, max_plies, counts.ctypes.data, fh.ctypes.data if trace else None,
+            pl.ctypes.data if trace else None))
+        return (counts, fh, pl) if trace else counts
+
+    def _ownership_dev(self, K, seed, max_plies, out):
+        import torch
+
+        dev = torch.device("cuda", self.device)
+        n = self.board_size
+        if out.dtype != torch.int32 or tuple(out.shape) != (self.num_games, 2, n * n) or not out.is_contiguous() \
+                or out.device != dev:
+            raise ValueError(f"out must be a contiguous int32 tensor of shape ({self.num_games}, 2, {n * n}) on {dev}")
+        if getattr(self, "_own_ev", None) is None:
+            self._own_ev = [torch.cuda.Event() for _ in range(2)]
+            self._own_stream = torch.cuda.ExternalStream(self.stream, device=dev)
+        ev, s = self._own_ev, self._own_stream
+        cur = torch.cuda.current_stream(dev)
+        ev[0].record(cur)
+        s.wait_event(ev[0])
+        _l.check(self._lib, self._lib.elfb200_ownership_dev(self._ctx, K, seed, max_plies, out.data_ptr()))
+        ev[1].record(s)
+        cur.wait_event(ev[1])
+        return out
+
+    def final_status(self, counts=None, playouts=None, threshold=0.5):
+        """dead groups and getTrompTaylorScore of every stored position.  With ``counts`` (``ownership``'s
+        result over ``playouts`` playouts) a group is dead when its stones' mean ownership margin for its own
+        colour, (own - opponent) / playouts, is below ``-threshold``; without counts no group is dead.  Returns
+        ``(dead, territory, score)``: uint8 ``[G, N*N]`` 1 on dead stones, uint8 ``[G, N*N]`` 1 black / 2 white /
+        3 dame with dead stones counted for the opponent, int32 ``[G]`` black minus white (no komi)."""
+        n, G = self.board_size, self.num_games
+        c = None
+        K = 0
+        if counts is not None:
+            if playouts is None:
+                raise ValueError("playouts is required with counts")
+            c = np.ascontiguousarray(counts, dtype=np.int32)
+            assert c.shape == (G, 2, n * n)
+            K = int(playouts)
+        dead = np.empty((G, n * n), np.uint8)
+        terr = np.empty((G, n * n), np.uint8)
+        score = np.empty(G, np.int32)
+        _l.check(self._lib, self._lib.elfb200_final_status(
+            self._ctx, c.ctypes.data if c is not None else None, K, float(threshold), dead.ctypes.data,
+            terr.ctypes.data, score.ctypes.data))
+        return dead, terr, score
 
     def launch_count(self):
         return self._lib.elfb200_launch_count(self._ctx)

@@ -16,6 +16,12 @@ Beyond ``console_lib.py``, three GTP 2 commands start a handicap game: ``fixed_h
 ``set_free_handicap v1 v2 ...``.  They need an empty board and a board that can take handicap stones
 (``GoBatch.place_handicap``); afterwards white is to move.
 
+``final_status_list alive|dead|seki`` (GTP 2) lists the groups of the position the game ended in, one group
+per line (vertices ascending, groups by their lowest vertex).  Dead groups come from Monte-Carlo ownership
+(``OnlineGame.final_status``: 1024 random playouts from the position); ``seki`` is always empty, there is no
+seki detection.  It is offered when the board behind the game can play those playouts
+(``GoBatch.ownership``).
+
 The reference console talks to its game thread by returning special actions from the
 ``human_actor`` callback; here the same special actions go straight into ``OnlineGame.human``.
 (The unmodified reference console can also be run against this engine through
@@ -55,6 +61,9 @@ class GtpConsole:
         if getattr(game.board, "place_handicap", None) is None:  # a board that cannot take handicap stones
             for k in HANDICAP_COMMANDS:
                 del self.commands[k]
+        if getattr(game.board, "ownership", None) is None:  # a board that cannot play ownership playouts
+            del self.commands["final_status_list"]
+        self.final_status_playouts = 1024
 
     # -- helpers ---------------------------------------------------------------------------------
     def check_player(self, player):  # console_lib.py:313-325
@@ -161,6 +170,17 @@ class GtpConsole:
         if len(acts) < 2 or not self.game.place_handicap(acts):  # a stone the board refuses: nothing placed
             return False, "bad vertex list"
         return True, ""
+
+    # -- end of game (GTP 2 section 6.3.5) ---------------------------------------------------------
+    def on_final_status_list(self, items):
+        status = items[1].lower() if len(items) > 1 else ""
+        if status not in ("alive", "dead", "seki"):
+            return False, "syntax error"
+        if status == "seki":  # no seki detection
+            return True, ""
+        dead, alive = self.game.final_status(playouts=self.final_status_playouts)
+        groups = dead if status == "dead" else alive
+        return True, "\n".join(" ".join(_o.action2vertex(a, self.board_size) for a in g) for g in groups)
 
     def on_final_score(self, items):
         s = self.game.getLastScore()

@@ -390,4 +390,12 @@ struct elfb200_ctx {
   // move lists of elfb200_replay (grown on demand)
   int16_t* d_replay = nullptr;
   size_t d_replay_bytes = 0;
+  // Monte-Carlo ownership and final status (elfb200_ownership / elfb200_final_status), allocated on first use
+  uint64_t* d_own_sk = nullptr;      // superko record of each game segment of k_ownership's resident grid
+  size_t d_own_sk_bytes = 0;
+  int32_t* d_own_counts = nullptr;   // G * 2 * N*N counts of the synchronous forms
+  uint8_t* d_own_status = nullptr;   // G * N*N dead flags, then G * N*N territory
+  uint64_t* d_own_hash = nullptr;    // per-playout final hash / plies of the synchronous form (grown on demand)
+  int32_t* d_own_plies = nullptr;
+  size_t d_own_trace = 0;            // playouts the two buffers above hold
 };

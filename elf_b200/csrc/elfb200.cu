@@ -9,6 +9,8 @@
 //   k_playout   whole random-policy games with the position (and the incremental safe/atari group
 //               masks) held in registers; to-terminal and steady-state ("stream") modes
 //   k_gather    copy games from another batch (GoState's copy constructor); no geometry, one kernel for both sizes
+//   k_ownership K random-policy playouts from every stored position, per-point area counts (Monte-Carlo ownership)
+//   k_final_status  dead groups from those counts, getTrompTaylorScore with them (territory map and score)
 //
 // HBM layout (structure of arrays, G games):
 //   cur   uint64 [G][N]      current position, row y = black_row | white_row << 32
@@ -840,6 +842,205 @@ __global__ void __launch_bounds__(GATHER_THREADS)
   }
 }
 
+// ---------------------------------------------------------------------------------------
+// Monte-Carlo ownership: K random-policy playouts from every stored position (elfb200_ownership).  Playout
+// j = g*K + k starts from game g's stored position and plays k_playout's policy with draw id j (candidate
+// pp_pick(seed, j, ply, n) of the legal non-eye moves of the side to move, a pass when there is none) until
+// GoState::terminated() or max_plies moves.  Its superko test covers game g's record and its own new pre-move
+// hashes, as GoState::forward on a copy of the game would.  A game that ended by two passes is played on with
+// an empty last-move window; one that ended by superko or the ply cap plays no move.  The stored games are
+// only read.
+//
+// counts[g][0][a] / counts[g][1][a] (a = x*N+y, zeroed by the host) count the playouts of game g whose final
+// position has point a in black's / white's area in simple_tt_scoring's view: stones, plus empties reachable
+// from them through empties only (the empties reachable from both colours count for neither).  Integer
+// atomics: the sums do not depend on the order in which playouts finish.
+//
+// k_playout's lane layout and stream mode, with a bounded scratch: a fixed grid of resident warps whose game
+// segments stride over the G*K playouts (segment s plays j = s, s + S, s + 2S, ...; S = segments in the grid).
+// A segment owns scratch[s][0 .. 2N^2), its superko record: a playout starts by copying game g's record
+// sk[g][0 .. sk_n) there and into the segment's Bloom filter, then appends its own pre-move hashes.
+template <int N>
+__global__ void __launch_bounds__(PLAYOUT_WARPS * 32)
+    k_ownership(DevState st, int K, uint64_t seed, int max_plies, uint64_t* __restrict__ scratch,
+                int32_t* __restrict__ counts, uint64_t* __restrict__ out_hash, int32_t* __restrict__ out_plies) {
+  constexpr int P = Geo<N>::P, MAXP = Geo<N>::MAX_PLY;
+  __shared__ uint64_t s_zob[Geo<N>::ZOB];
+  __shared__ uint32_t s_bloom[PLAYOUT_WARPS][Geo<N>::GPW][128];  // as in k_playout
+  load_zobrist<N>(s_zob);
+  const Lane L = make_lane<N>();
+  const int64_t total = (int64_t)st.G * K;
+  const int64_t nseg = (int64_t)gridDim.x * PLAYOUT_WARPS * Geo<N>::GPW;
+  const int seg = ((blockIdx.x * blockDim.x + threadIdx.x) >> 5) * Geo<N>::GPW + L.sub;
+  uint64_t* skg = scratch + (size_t)seg * MAXP;
+  uint32_t* bloom = s_bloom[threadIdx.x >> 5][L.sub];
+
+  int64_t j = L.active ? seg : total;  // this segment's playout
+  uint32_t b = 0, w = 0, safe = 0, atari = 0;
+  BoardMeta meta = initial_meta();
+  uint64_t hash = 0;
+  int nsk = 0, t = 0;
+  bool have = false, load = j < total;
+
+  while (true) {
+    if (__any_sync(FULL, load)) {  // segments whose playout finished start their next one
+      if (load)
+        for (int i = L.row; i < 128; i += N) bloom[i] = 0u;
+      __syncwarp();
+      if (load) {
+        const int g = (int)(j / K);
+        const uint64_t rv = st.cur[(size_t)g * N + L.row], sav = st.sa[(size_t)g * N + L.row];
+        b = (uint32_t)rv;
+        w = (uint32_t)(rv >> 32);
+        safe = (uint32_t)sav;
+        atari = (uint32_t)(sav >> 32);
+        meta = load_meta(&st.meta[g]);
+        hash = st.hash[g];
+        nsk = st.sk_n[g];
+        if (meta.last1 == MV_PASS && meta.last2 == MV_PASS) meta.last1 = meta.last2 = MV_INVALID;
+        const uint64_t* src = st.sk + (size_t)g * MAXP;
+        for (int i = L.row; i < nsk; i += N) {
+          const uint64_t h = src[i];
+          skg[i] = h;
+          const uint32_t i1 = (uint32_t)h & 4095u, i2 = (uint32_t)(h >> 12) & 4095u;
+          atomicOr(&bloom[i1 >> 5], 1u << (i1 & 31));
+          atomicOr(&bloom[i2 >> 5], 1u << (i2 & 31));
+        }
+        t = 0;
+        have = true;
+        load = false;
+      }
+      __syncwarp();
+    }
+    const bool over = have && (is_terminated<N>(meta) || t >= max_plies);
+    if (__any_sync(FULL, over)) {  // area of the final positions (tt_score's fill, a warp collective)
+      const uint32_t e = ~(b | w) & L.rm;
+      uint32_t ar[2] = {b, w};
+      const uint32_t thr[2] = {e, e};
+      floodK<N, 2>(ar, thr, L);
+      if (over) {
+        int32_t* cg = counts + (size_t)(j / K) * 2 * P;
+        uint32_t ab = ar[0] & ~ar[1], aw = ar[1] & ~ar[0];
+        while (ab) {
+          const int x = __ffs(ab) - 1;
+          ab &= ab - 1;
+          atomicAdd(cg + x * N + L.row, 1);
+        }
+        while (aw) {
+          const int x = __ffs(aw) - 1;
+          aw &= aw - 1;
+          atomicAdd(cg + P + x * N + L.row, 1);
+        }
+        if (L.row == 0) {
+          if (out_hash) out_hash[j] = hash;
+          if (out_plies) out_plies[j] = t;
+        }
+        j += nseg;
+        have = false;
+        load = j < total;
+      }
+      continue;
+    }
+    if (__all_sync(FULL, !have)) break;
+    // one ply of k_playout's policy
+    const bool term = !have;
+    const uint32_t own = meta.next == S_BLACK ? b : w, opp = meta.next == S_BLACK ? w : b;
+    const bool ko_applies = (meta.flags & F_KO_ACTIVE) && meta.ko_color == meta.next;
+    const uint32_t legal = legal_rows_cached<N>(own, opp, safe, atari, L, ko_applies, meta.ko_pt);
+    const uint32_t cand = legal & ~true_eye_rows<N>(own, opp, L);
+    const int n = game_sum<N>(__popc(cand), L);
+    const int k = n > 0 ? (int)pp_pick(seed, (uint64_t)j, meta.ply, (uint32_t)n) : 0;
+    const int p = select_kth_action_order<N>(cand, k, L);
+    const int pm = term ? MV_NONE : (n > 0 ? p : MV_PASS);
+    const uint64_t pre_hash = hash;
+    play_move_cached<N>(b, w, meta, hash, pm, s_zob, L, safe, atari);
+    const uint32_t q1 = (uint32_t)hash & 4095u, q2 = (uint32_t)(hash >> 12) & 4095u;
+    const bool maybe = pm >= 0 && ((bloom[q1 >> 5] >> (q1 & 31)) & (bloom[q2 >> 5] >> (q2 & 31)) & 1u);
+    bool sko = false;
+    if (__any_sync(FULL, maybe)) sko = superko_scan<N>(skg, maybe ? nsk : 0, hash, L);
+    __syncwarp();
+    if (pm >= 0) {
+      if (sko) meta.flags |= F_SUPERKO;
+      if (L.row == 0) {
+        skg[nsk] = pre_hash;
+        const uint32_t i1 = (uint32_t)pre_hash & 4095u, i2 = (uint32_t)(pre_hash >> 12) & 4095u;
+        bloom[i1 >> 5] |= 1u << (i1 & 31);
+        bloom[i2 >> 5] |= 1u << (i2 & 31);
+      }
+      nsk++;
+    }
+    if (!term) t++;
+    __syncwarp();
+  }
+}
+
+// ---------------------------------------------------------------------------------------
+// Dead groups and getTrompTaylorScore (board.cc:1954-2071) of every stored position (elfb200_final_status).
+// One warp per game (row per lane, make_lane_single), groups found one at a time by link-masked fills.
+//
+// Dead rule (ours, not the reference's: it leaves the choice of dead groups to its caller): with the ownership
+// counts of K playouts, a group S of colour c is dead iff
+//   own(S) = sum over p in S of (c == black ? counts_b[p] - counts_w[p] : counts_w[p] - counts_b[p])
+//   satisfies  (double)own(S) < -threshold * K * |S|.
+// Without counts no group is dead.  Dead groups are counted for the opponent (S_DEAD in group_stats): every
+// stone takes its (flipped) colour, an empty region the one colour among the stones it touches, else 3 (dame;
+// also every point of the empty board).  score = black points - white points.
+template <int N>
+__global__ void __launch_bounds__(32)
+    k_final_status(DevState st, const int32_t* __restrict__ counts, int K, double threshold,
+                   uint8_t* __restrict__ dead_out, uint8_t* __restrict__ terr_out, int32_t* __restrict__ score_out) {
+  constexpr int P = Geo<N>::P;
+  const Lane L = make_lane_single<N>();
+  const int g = blockIdx.x;
+  const uint64_t rv = L.active ? st.cur[(size_t)g * N + L.row] : 0ull;
+  const uint32_t b = (uint32_t)rv, w = (uint32_t)(rv >> 32);
+  uint32_t dead = 0;
+  if (counts) {
+    const int32_t* cb = counts + (size_t)g * 2 * P;
+    const int32_t* cw = cb + P;
+    const Links lk = make_links<N>(b, w, L);
+    uint32_t left = b | w;
+    while (true) {
+      const unsigned lanes = __ballot_sync(FULL, left != 0u);
+      if (!lanes) break;
+      const int src = __ffs(lanes) - 1;  // seed: the lowest stone of the first row that has one left
+      const uint32_t seed_bit = __shfl_sync(FULL, left & (0u - left), src);
+      const bool black = __shfl_sync(FULL, (seed_bit & b) ? 1 : 0, src) != 0;
+      uint32_t grp = L.lane == src ? seed_bit : 0u;
+      while (true) {
+        const uint32_t n2 = grow_link(grow_link(grp, lk), lk);
+        const bool ch = n2 != grp;
+        grp = n2;
+        if (!__any_sync(FULL, ch)) break;
+      }
+      long long own = 0;
+      for (uint32_t m = grp; m; m &= m - 1) {
+        const int a = (__ffs(m) - 1) * N + L.row;
+        own += black ? (long long)cb[a] - cw[a] : (long long)cw[a] - cb[a];
+      }
+      for (int o = 16; o; o >>= 1) own += __shfl_xor_sync(FULL, own, o);
+      const int size = game_sum<N>(__popc(grp), L);
+      if ((double)own < -threshold * (double)K * (double)size) dead |= grp;
+      left &= ~grp;
+    }
+  }
+  const uint32_t bf = (b & ~dead) | (w & dead), wf = (w & ~dead) | (b & dead);
+  const uint32_t e = ~(bf | wf) & L.rm;
+  uint32_t ar[2] = {bf, wf};
+  const uint32_t thr[2] = {e, e};
+  floodK<N, 2>(ar, thr, L);
+  const uint32_t tb = ar[0] & ~ar[1], tw = ar[1] & ~ar[0];
+  const int score = game_sum<N>(__popc(tb) - __popc(tw), L);
+  if (L.active) {
+    for (int x = 0; x < N; ++x) {
+      const size_t a = (size_t)g * P + x * N + L.row;
+      if (dead_out) dead_out[a] = (uint8_t)((dead >> x) & 1u);
+      if (terr_out) terr_out[a] = (uint8_t)(((tb >> x) & 1u) ? S_BLACK : ((tw >> x) & 1u) ? S_WHITE : 3);
+    }
+  }
+  if (L.lane == 0 && score_out) score_out[g] = score;
+}
+
 }  // namespace elfb200
 
 // =========================================================================================
@@ -951,7 +1152,8 @@ void elfb200_destroy(elfb200_ctx* c) {
   void* ptrs[] = {c->st.cur,  c->st.ring, c->st.legal, c->st.hash,   c->st.meta,   c->st.sk,
                   c->st.sk_n, c->d_actions, c->d_ok,   c->d_bytes,   c->d_words,   c->d_d4,
                   c->d_feat,  c->d_po_sk, c->d_po_chk, c->d_po_hash, c->d_po_plies, c->d_po_score,
-                  c->d_replay, c->st.placed, c->st.sa, c->d_exp_table, c->d_done};
+                  c->d_replay, c->st.placed, c->st.sa, c->d_exp_table, c->d_done,
+                  c->d_own_sk, c->d_own_counts, c->d_own_status, c->d_own_hash, c->d_own_plies};
   for (void* p : ptrs)
     if (p) cudaFree(p);
   if (c->h_pin) cudaFreeHost(c->h_pin);
@@ -1450,6 +1652,127 @@ int elfb200_playout(elfb200_ctx* c, uint64_t seed, uint64_t first_game_id, int m
   int rc = elfb200_playout_launch(c, seed, first_game_id, max_plies);
   if (rc) return rc;
   return elfb200_playout_results(c, chk_host, plies_host, score_host, final_hash_host, total_plies);
+}
+
+}  // extern "C"
+
+// ---- Monte-Carlo ownership and final status ------------------------------------------------------------------
+static int check_ownership(const elfb200_ctx* c, int playouts, int max_plies, const void* counts) {
+  if (!c) return elfb200_fail(ELFB200_ERR_ARG, "ctx is NULL");
+  if (!counts) return elfb200_fail(ELFB200_ERR_ARG, "counts is NULL");
+  if (playouts < 1) return elfb200_fail(ELFB200_ERR_ARG, "playouts must be at least 1 (got %d)", playouts);
+  if ((int64_t)c->G * playouts > INT32_MAX)
+    return elfb200_fail(ELFB200_ERR_ARG, "%d games x %d playouts exceed INT32_MAX", c->G, playouts);
+  if (max_plies < 0) return elfb200_fail(ELFB200_ERR_ARG, "max_plies must not be negative (got %d)", max_plies);
+  return ELFB200_OK;
+}
+
+// k_ownership on the context stream: counts zeroed, then a grid of at most the warps the device holds at once,
+// each segment with a superko scratch of 2N^2 words (allocated on first use, grown with the grid).
+template <int N>
+static int ownership_launch(elfb200_ctx* c, int K, uint64_t seed, int max_plies, int32_t* counts, uint64_t* hash,
+                            int32_t* plies) {
+  constexpr int GPW = Geo<N>::GPW;
+  const int64_t total = (int64_t)c->G * K;
+  int64_t warps = (total + GPW - 1) / GPW;
+#if defined(ELFB200_SIMT_EMU)
+  const int64_t resident = 2;  // few warps, each striding over many playouts
+#else
+  int sms = 0, per_sm = 0;
+  CK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, c->device));
+  CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_ownership<N>, PLAYOUT_WARPS * 32, 0));
+  const int64_t resident = (int64_t)sms * (per_sm > 0 ? per_sm : 1) * PLAYOUT_WARPS;
+#endif
+  if (warps > resident) warps = resident;
+  const int grid = (int)((warps + PLAYOUT_WARPS - 1) / PLAYOUT_WARPS);
+  const size_t sk_bytes = (size_t)grid * PLAYOUT_WARPS * GPW * Geo<N>::MAX_PLY * sizeof(uint64_t);
+  if (sk_bytes > c->d_own_sk_bytes) {
+    if (c->d_own_sk) CK(cudaFree(c->d_own_sk));
+    c->d_own_sk = nullptr;
+    c->d_own_sk_bytes = 0;
+    CK(cudaMalloc(&c->d_own_sk, sk_bytes));
+    c->d_own_sk_bytes = sk_bytes;
+  }
+  CK(cudaMemsetAsync(counts, 0, (size_t)c->G * 2 * Geo<N>::P * sizeof(int32_t), c->stream));
+  k_ownership<N><<<grid, PLAYOUT_WARPS * 32, 0, c->stream>>>(c->st, K, seed, max_plies, c->d_own_sk, counts, hash,
+                                                             plies);
+  c->launches++;
+  CK(cudaGetLastError());
+  return ELFB200_OK;
+}
+
+extern "C" {
+
+int elfb200_ownership_dev(elfb200_ctx* c, int playouts, uint64_t seed, int max_plies, int32_t* counts_dev) {
+  int rc = check_ownership(c, playouts, max_plies, counts_dev);
+  if (rc) return rc;
+  CK(cudaSetDevice(c->device));
+  DISPATCH_N(c, (rc = ownership_launch<19>(c, playouts, seed, max_plies, counts_dev, nullptr, nullptr)),
+             (rc = ownership_launch<9>(c, playouts, seed, max_plies, counts_dev, nullptr, nullptr)));
+  return rc;
+}
+
+int elfb200_ownership(elfb200_ctx* c, int playouts, uint64_t seed, int max_plies, int32_t* counts_host,
+                      uint64_t* final_hash_host, int32_t* plies_host) {
+  int rc = check_ownership(c, playouts, max_plies, counts_host);
+  if (rc) return rc;
+  CK(cudaSetDevice(c->device));
+  const size_t P = (size_t)c->N * c->N, total = (size_t)c->G * playouts;
+  if (!c->d_own_counts) CK(cudaMalloc(&c->d_own_counts, (size_t)c->G * 2 * P * sizeof(int32_t)));
+  const bool trace = final_hash_host || plies_host;
+  if (trace && total > c->d_own_trace) {
+    if (c->d_own_hash) CK(cudaFree(c->d_own_hash));
+    if (c->d_own_plies) CK(cudaFree(c->d_own_plies));
+    c->d_own_hash = nullptr;
+    c->d_own_plies = nullptr;
+    c->d_own_trace = 0;
+    CK(cudaMalloc(&c->d_own_hash, total * sizeof(uint64_t)));
+    CK(cudaMalloc(&c->d_own_plies, total * sizeof(int32_t)));
+    c->d_own_trace = total;
+  }
+  uint64_t* dh = final_hash_host ? c->d_own_hash : nullptr;
+  int32_t* dp = plies_host ? c->d_own_plies : nullptr;
+  DISPATCH_N(c, (rc = ownership_launch<19>(c, playouts, seed, max_plies, c->d_own_counts, dh, dp)),
+             (rc = ownership_launch<9>(c, playouts, seed, max_plies, c->d_own_counts, dh, dp)));
+  if (rc) return rc;
+  CK(cudaMemcpyAsync(counts_host, c->d_own_counts, (size_t)c->G * 2 * P * sizeof(int32_t), cudaMemcpyDeviceToHost,
+                     c->stream));
+  if (dh) CK(cudaMemcpyAsync(final_hash_host, dh, total * sizeof(uint64_t), cudaMemcpyDeviceToHost, c->stream));
+  if (dp) CK(cudaMemcpyAsync(plies_host, dp, total * sizeof(int32_t), cudaMemcpyDeviceToHost, c->stream));
+  CK(cudaStreamSynchronize(c->stream));
+  return ELFB200_OK;
+}
+
+int elfb200_final_status(elfb200_ctx* c, const int32_t* counts_host, int playouts, double threshold,
+                         uint8_t* dead_host, uint8_t* territory_host, int32_t* score_host) {
+  if (!c) return elfb200_fail(ELFB200_ERR_ARG, "ctx is NULL");
+  if (counts_host && playouts < 1)
+    return elfb200_fail(ELFB200_ERR_ARG, "playouts must be at least 1 (got %d)", playouts);
+  if (counts_host && (int64_t)c->G * playouts > INT32_MAX)
+    return elfb200_fail(ELFB200_ERR_ARG, "%d games x %d playouts exceed INT32_MAX", c->G, playouts);
+  if (!std::isfinite(threshold)) return elfb200_fail(ELFB200_ERR_ARG, "threshold must be finite");
+  CK(cudaSetDevice(c->device));
+  const size_t P = (size_t)c->N * c->N, G = c->G;
+  if (!c->d_own_status) CK(cudaMalloc(&c->d_own_status, G * 2 * P));
+  const int32_t* dcounts = nullptr;
+  if (counts_host) {
+    if (!c->d_own_counts) CK(cudaMalloc(&c->d_own_counts, G * 2 * P * sizeof(int32_t)));
+    CK(cudaMemcpyAsync(c->d_own_counts, counts_host, G * 2 * P * sizeof(int32_t), cudaMemcpyHostToDevice, c->stream));
+    dcounts = c->d_own_counts;
+  }
+  uint8_t* ddead = c->d_own_status;
+  uint8_t* dterr = c->d_own_status + G * P;
+  DISPATCH_N(c, (k_final_status<19><<<c->G, 32, 0, c->stream>>>(c->st, dcounts, playouts, threshold, ddead, dterr,
+                                                                c->d_words)),
+             (k_final_status<9><<<c->G, 32, 0, c->stream>>>(c->st, dcounts, playouts, threshold, ddead, dterr,
+                                                               c->d_words)));
+  c->launches++;
+  CK(cudaGetLastError());
+  if (dead_host) CK(cudaMemcpyAsync(dead_host, ddead, G * P, cudaMemcpyDeviceToHost, c->stream));
+  if (territory_host) CK(cudaMemcpyAsync(territory_host, dterr, G * P, cudaMemcpyDeviceToHost, c->stream));
+  if (score_host) CK(cudaMemcpyAsync(score_host, c->d_words, G * sizeof(int32_t), cudaMemcpyDeviceToHost, c->stream));
+  CK(cudaStreamSynchronize(c->stream));
+  return ELFB200_OK;
 }
 
 }  // extern "C"

@@ -60,6 +60,9 @@ SIGNATURES = {
     "elfb200_playout_launch": (ctypes.c_int, [vp, ctypes.c_uint64, ctypes.c_uint64, ctypes.c_int]),
     "elfb200_playout_results": (ctypes.c_int, [vp, vp, vp, vp, vp, vp]),
     "elfb200_launch_count": (ctypes.c_int64, [vp]),
+    "elfb200_ownership": (ctypes.c_int, [vp, ctypes.c_int, ctypes.c_uint64, ctypes.c_int, vp, vp, vp]),
+    "elfb200_ownership_dev": (ctypes.c_int, [vp, ctypes.c_int, ctypes.c_uint64, ctypes.c_int, vp]),
+    "elfb200_final_status": (ctypes.c_int, [vp, vp, ctypes.c_int, ctypes.c_double, vp, vp, vp]),
     "elfb200_playout_stream": (ctypes.c_int, [vp, ctypes.c_uint64, ctypes.c_uint64, ctypes.c_int, vp, vp, vp, vp, vp]),
     "elfb200_playout_stream_launch": (ctypes.c_int, [vp, ctypes.c_uint64, ctypes.c_uint64, ctypes.c_int]),
     # include/elfb200_mcts.h

@@ -106,6 +106,29 @@ def show_board(stones, n, last_action, b_cap, w_cap, next_player):
     return "".join(out) + "\nLast move: " + last + ", nextPlayer: " + ("Black" if next_player == S_BLACK else "White") + "\n"
 
 
+def stone_groups(stones, n):
+    """the groups (4-connected stones of one colour) of a position given as colours by action x*N+y: lists of
+    actions in ascending order, ordered by their lowest action"""
+    seen = np.zeros(n * n, bool)
+    groups = []
+    for a in range(n * n):
+        if stones[a] == 0 or seen[a]:
+            continue
+        grp, todo = [], [a]
+        seen[a] = True
+        while todo:
+            p = todo.pop()
+            grp.append(p)
+            x, y = divmod(p, n)
+            for q in ((p - n) if x > 0 else -1, (p + n) if x < n - 1 else -1, (p - 1) if y > 0 else -1,
+                      (p + 1) if y < n - 1 else -1):
+                if q >= 0 and not seen[q] and stones[q] == stones[a]:
+                    seen[q] = True
+                    todo.append(q)
+        groups.append(sorted(grp))
+    return groups
+
+
 class OnlineGame:
     def __init__(self, board, search, komi=7.5, resign_thres=0.0, policy_distri_cutoff=0, move_cutoff=-1,
                  preload_sgf=None, preload_sgf_move_to=-1, following_pass=False, seed=0):
@@ -128,6 +151,8 @@ class OnlineGame:
         self._sgf = None
         self._sgf_pos = 0
         self._preload = (preload_sgf, int(preload_sgf_move_to))
+        self._final = None  # one-game batch holding the position of the last finished game
+        self._final_kept = False
         self._restart(first=True)
 
     @classmethod
@@ -213,8 +238,38 @@ class OnlineGame:
             self._last_move_of_finished = int(i[4])
         self.last_value = fv
         self.finished.append((fv, int(i[0]), reason))
+        self._keep_final_position()
         self._restart_game()
         return fv
+
+    def _keep_final_position(self):
+        """copy the finished position into a one-game batch before the restart, so ``final_status`` can still
+        look at it (boards that cannot copy games keep nothing)"""
+        if getattr(self.board, "gather", None) is None:
+            return
+        if self._final is None:
+            self._final = self.board.new_like(1)
+        self._final.gather(self.board, [0])
+        self._final_kept = True
+
+    # -- end of game: dead stones -------------------------------------------------------------------
+    def final_status(self, playouts=1024, seed=0, threshold=0.5):
+        """dead and alive groups of the position the game ended in: the kept final position when the board
+        was restarted after a finished game and nothing has been played since, the current position otherwise.
+        A group is dead when ``playouts`` random playouts from the position leave its stones, on average, more
+        than ``threshold`` in the opponent's area (``GoBatch.ownership`` / ``GoBatch.final_status``).  Returns
+        ``(dead, alive)``: lists of groups, each a list of actions (x*N+y) in ascending order, the groups
+        ordered by their lowest action."""
+        board = self.board
+        i = self.info()
+        if self._final_kept and int(i[0]) == 1 and not board.stones()[0].any():
+            board = self._final
+        counts = board.ownership(playouts, seed=seed)
+        dead = board.final_status(counts, playouts, threshold)[0][0]
+        dead_groups, alive_groups = [], []
+        for grp in stone_groups(board.stones()[0], self.N):
+            (dead_groups if dead[grp[0]] else alive_groups).append(grp)
+        return dead_groups, alive_groups
 
     # -- handicap -----------------------------------------------------------------------------------
     def place_handicap(self, actions):

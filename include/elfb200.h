@@ -172,6 +172,31 @@ int elfb200_playout_stream_launch(elfb200_ctx* ctx, uint64_t seed, uint64_t firs
  * 1.35 vs 1.00 G at 12,288), one row per lane below.  Same results either way. */
 int elfb200_set_playout_layout(elfb200_ctx* ctx, int layout);
 
+/* Monte-Carlo ownership of the stored positions: for every game g, `playouts` (K) random playouts of the policy
+ * of include/elfb200_playout_policy.h start from g's position (playout k uses draw id g*K + k), each played with
+ * GoState::forward on a copy of g's GoState (go_state.h:117-124) until GoState::terminated() -- superko against
+ * g's record and the playout's own moves -- or `max_plies` moves (>= 0).  A game that ended by
+ * two passes is played on with an empty last-move window (Board::_last_move/_last_move2); one that ended by
+ * superko or the ply cap plays no move.  counts int32[G][2][N*N] (zeroed by the call), by action x*N+y: the
+ * playouts whose final position has the point in black's [0] / white's [1] area as simple_tt_scoring
+ * (go_state.h:75-93) sees it.  Integer sums: bit-for-bit the same for a seed.  The stored games are not changed.
+ * final_hash uint64[G][K] and plies int32[G][K] (each may be NULL): every playout's final GoState::getHashCode
+ * and moves played.  Synchronous.  G*K <= INT32_MAX. */
+int elfb200_ownership(elfb200_ctx* ctx, int playouts, uint64_t seed, int max_plies, int32_t* counts_host,
+                      uint64_t* final_hash_host, int32_t* plies_host);
+/* The same counts into device memory, asynchronous on the context stream and capturable once a first call has
+ * allocated the per-warp superko scratch (the same board size and at least as many playouts in all). */
+int elfb200_ownership_dev(elfb200_ctx* ctx, int playouts, uint64_t seed, int max_plies, int32_t* counts_dev);
+/* getTrompTaylorScore(board, group_stats, territory) (board.cc:1954-2071, board.h:431-445) of every stored position
+ * with the groups this call finds dead flagged S_DEAD in group_stats.  Dead (a heuristic, not the reference's: it
+ * leaves the choice to its caller): with the counts of elfb200_ownership over `playouts` (K) playouts, a group S of
+ * colour c is dead iff sum over S of (own area count - opponent area count) < -threshold * K * |S|; with
+ * counts_host == NULL no group is dead.  dead uint8[G][N*N] (1 on every stone of a dead group), territory
+ * uint8[G][N*N] (1 black, 2 white, 3 dame; stones of dead groups count for the opponent), score int32[G] (black
+ * minus white, no komi; simple_tt_scoring when no group is dead).  Outputs may be NULL.  Synchronous. */
+int elfb200_final_status(elfb200_ctx* ctx, const int32_t* counts_host, int playouts, double threshold,
+                         uint8_t* dead_host, uint8_t* territory_host, int32_t* score_host);
+
 /* Number of kernels this library has launched since creation (bench gpu_launches).  Counts enqueues by
  * the calls above; replays of a CUDA graph that captured them are not counted. */
 int64_t elfb200_launch_count(const elfb200_ctx* ctx);
