@@ -91,6 +91,10 @@ __device__ __forceinline__ int game_sum(int v, const Lane2& L) {
   const uint32_t r = __reduce_add_sync(FULL, L.active ? ((uint32_t)v << L.shift) : 0u);
   return (int)((r >> L.shift) & 1023u);
 }
+template <int N>  // board.cuh's spelling, for code written for both layouts
+__device__ __forceinline__ int game_sum(int v, const Lane2& L) {
+  return game_sum(v, L);
+}
 template <int N>
 __device__ __forceinline__ uint64_t game_xor64(uint64_t v, const Lane2& L) {
   uint32_t lo = 0, hi = 0;
