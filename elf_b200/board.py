@@ -357,5 +357,50 @@ class GoBatch:
             terr.ctypes.data, score.ctypes.data))
         return dead, terr, score
 
+    # -- ladders and self-ataris ---------------------------------------------------------------
+    def tactics(self, out=None, trace=False):
+        """the reference's checkLadder and isSelfAtari for every point and both colours (index 0 black, 1 white),
+        whoever is to move, by action x*N+y.  Returns ``(ladder, self_atari)``, int16 ``[G, 2, N*N]`` each:
+        the depth at which the group escaping by that move is caught in a ladder (0: no ladder, or an illegal
+        move), and the stones of the group the move leaves in atari (0: not a self-atari).  ``trace=True`` adds
+        ``calls``, int32 ``[G, 2, N*N]``: how many search calls each ladder read took (0 where none ran).  With
+        ``out=(ladder, self_atari)``, contiguous int16 CUDA tensors of shape ``[G, 2, N*N]`` on this batch's
+        device (either may be None, and its work is skipped), the values are written there asynchronously,
+        ordered after the caller's current stream and before its next work with events only (capturable in a
+        CUDA graph); ``out`` is returned.  The stored games stay as they are."""
+        n, G = self.board_size, self.num_games
+        if out is not None:
+            return self._tactics_dev(out)
+        ladder = np.empty((G, 2, n * n), np.int16)
+        sa = np.empty((G, 2, n * n), np.int16)
+        calls = np.empty((G, 2, n * n), np.int32) if trace else None
+        _l.check(self._lib, self._lib.elfb200_tactics(self._ctx, ladder.ctypes.data, sa.ctypes.data,
+                                                      calls.ctypes.data if trace else None))
+        return (ladder, sa, calls) if trace else (ladder, sa)
+
+    def _tactics_dev(self, out):
+        import torch
+
+        dev = torch.device("cuda", self.device)
+        n = self.board_size
+        ladder, sa = out
+        for t in (ladder, sa):
+            if t is not None and (t.dtype != torch.int16 or tuple(t.shape) != (self.num_games, 2, n * n)
+                                  or not t.is_contiguous() or t.device != dev):
+                raise ValueError(f"out must hold contiguous int16 tensors of shape ({self.num_games}, 2, {n * n}) "
+                                 f"on {dev}, or None")
+        if getattr(self, "_tac_ev", None) is None:
+            self._tac_ev = [torch.cuda.Event() for _ in range(2)]
+            self._tac_stream = torch.cuda.ExternalStream(self.stream, device=dev)
+        ev, s = self._tac_ev, self._tac_stream
+        cur = torch.cuda.current_stream(dev)
+        ev[0].record(cur)
+        s.wait_event(ev[0])
+        _l.check(self._lib, self._lib.elfb200_tactics_dev(self._ctx, ladder.data_ptr() if ladder is not None else None,
+                                                          sa.data_ptr() if sa is not None else None))
+        ev[1].record(s)
+        cur.wait_event(ev[1])
+        return out
+
     def launch_count(self):
         return self._lib.elfb200_launch_count(self._ctx)

@@ -398,4 +398,6 @@ struct elfb200_ctx {
   uint64_t* d_own_hash = nullptr;    // per-playout final hash / plies of the synchronous form (grown on demand)
   int32_t* d_own_plies = nullptr;
   size_t d_own_trace = 0;            // playouts the two buffers above hold
+  // elfb200_tactics (synchronous form), allocated on first use: G*2*N*N int16 ladder, int16 self_atari, int32 calls
+  void* d_tac = nullptr;
 };

@@ -14,6 +14,7 @@
 //   k_gather    copy games from another batch (GoState's copy constructor); no geometry, one kernel for both sizes
 //   k_ownership K random-policy playouts from every stored position, per-point area counts (Monte-Carlo ownership)
 //   k_final_status  dead groups from those counts, getTrompTaylorScore with them (territory map and score)
+//   k_tactics   checkLadder and isSelfAtari for every point and both colours (ladder depth, self-atari size)
 //
 // Each game rule lives in one device function that the kernels share: forward_ply is GoState::forward's move
 // (k_step, k_env_step, k_replay), random_ply one move of the random policy (k_playout, k_playout2, k_ownership),
@@ -990,6 +991,252 @@ __global__ void __launch_bounds__(32)
   if (L.lane == 0 && score_out) score_out[g] = score;
 }
 
+// ---------------------------------------------------------------------------------------
+// Ladders and self-ataris (elfb200_tactics): for every stored position, every point p and both colours c,
+// whoever is to move, with ids = TryPlay(board, x, y, c) (board.cc:788-827; 0 where it refuses the move):
+//   ladder[g][c][a]     checkLadder(board, ids, c) (board.cc:476-524): the depth at which the group of colour c
+//                       that escapes by playing p is caught in checkLadderUseSearch (board.cc:299-439), 0 if none;
+//   self_atari[g][c][a] isSelfAtari(board, ids, p, c) (board.cc:242-297): the stones of the group the move
+//                       leaves with one liberty, 0 if it leaves none.
+// One warp per game, one board row per lane (make_lane_single); the stored games are only read.
+//
+// Candidates first, by mask operations on the whole board.  checkLadder searches only when p has exactly two
+// empty neighbours (ids->liberty == 2), exactly one own neighbour group, in atari, and exactly one enemy
+// neighbour group, with >= 3 liberties.  With two of the four neighbours empty the other two must be one own
+// stone and one enemy stone, so "empty, legal for c, two empty neighbours, next to a c stone in atari and to an
+// enemy stone" is exact up to the enemy group's liberty count, which one fill gives.  isSelfAtari needs at most
+// one empty neighbour; its early-outs agree with "play it and count the new group's liberties", which two fills
+// (the merged group, the captured groups) do without playing the move.
+//
+// The search is checkLadderUseSearch without recursion.  A node is the position after the moves path[0 .. len)
+// from the stored position (path[0] = p, the victim's move; depth = len).  Every node visited counts one call.
+// At a capturer node with two escapes and neither must be blocked, the reference plays escape[0] on a copy and
+// then escape[1] on the board itself: here escape[0] is played and (len, escape[1]) pushed as a pending branch.
+// A node that returns 0 makes every ancestor return 0 up to the deepest pending branch, which is popped: its
+// position is rebuilt by replaying path[0 .. len) from the stored position (Play is deterministic, and the
+// reference expects branching to "seldomly happen") and escape[1] is tried there.  Liberty counts that decide
+// (1 / 2 / >= 3) are exact: 1 from the atari mask, 2 and more from a group fill.  Moves go through TryPlay2:
+// empty, not suicide, not the simple-ko point of the player to move (no superko, no history: this is Board).
+// The path and the pending branches live in shared memory, TAC_MAX_PATH plies per warp; a search that would
+// pass that writes -1, a value the reference never returns.
+constexpr int TACTICS_WARPS = 4;      // games per CTA
+constexpr int LADDER_BUDGET = 1024;   // MAX_LADDER_SEARCH (board.cc:298)
+template <int N>
+struct Tac {
+  static constexpr int MAX_PATH = 2 * N * N;  // plies of one search
+  static constexpr int MAX_PEND = N * N;      // pending branches: capturer nodes are every second ply
+};
+
+// delta4 (board.h:220): (x-1, y), (x, y-1), (x+1, y), (x, y+1)
+__device__ __forceinline__ int d4x(int d) { return d == 0 ? -1 : d == 2 ? 1 : 0; }
+__device__ __forceinline__ int d4y(int d) { return d == 1 ? -1 : d == 3 ? 1 : 0; }
+
+// Point (x, y) of the row words v, false off the board.  Warp-uniform: every lane gets row y by a shuffle.
+template <int N>
+__device__ __forceinline__ bool bit_at(uint32_t v, int x, int y) {
+  const bool on = x >= 0 && x < N && y >= 0 && y < N;
+  const uint32_t r = __shfl_sync(FULL, v, on ? y : 0);
+  return on && ((r >> x) & 1u);
+}
+
+// Sum over the game's rows, the same on every lane of the warp (one game per warp, idle lanes add 0).
+__device__ __forceinline__ int warp_rows_sum(int v, const Lane& L) { return __reduce_add_sync(FULL, L.active ? v : 0); }
+
+// Exact liberty count of the group of `stones` on point (x, y).
+template <int N>
+__device__ __forceinline__ int group_libs(uint32_t stones, uint32_t empty, int x, int y, const Lane& L) {
+  const uint32_t seed = (L.active && L.row == y) ? (1u << x) : 0u;
+  const uint32_t grp = flood<N>(seed, stones, L);
+  return warp_rows_sum(__popc(nbr4<N>(grp, L) & empty), L);
+}
+
+// Directions d (bit d, delta4 order) in which (x, y) has an empty on-board neighbour.
+template <int N>
+__device__ __forceinline__ unsigned empty_dirs(uint32_t empty, int x, int y) {
+  unsigned m = 0;
+#pragma unroll
+  for (int d = 0; d < 4; ++d)
+    if (bit_at<N>(empty, x + d4x(d), y + d4y(d))) m |= 1u << d;
+  return m;
+}
+// the neighbour of point p in direction d
+template <int N>
+__device__ __forceinline__ int step4(int p, int d) { return p + d4x(d) + d4y(d) * N; }
+
+struct TacPos {
+  uint32_t b, w, safe, atari;
+  BoardMeta meta;
+  uint64_t hash;
+};
+
+template <int N>
+__device__ __forceinline__ void tac_play(TacPos& s, int p, const uint64_t* zob, const Lane& L) {
+  play_move_cached<N>(s.b, s.w, s.meta, s.hash, p, zob, L, s.safe, s.atari);
+}
+
+// TryPlay2 (board.cc:784-786) of point m for the player to move.
+template <int N>
+__device__ __forceinline__ bool tac_legal(const TacPos& s, int m, const Lane& L) {
+  return bit_at<N>(legal_for_next<N>(s.b, s.w, s.safe, s.atari, s.meta, L), m % N, m / N);
+}
+
+// checkLadder's search after the victim (colour of s0.meta.next) plays p on s0: the depth at which the victim is
+// caught, 0 if it is not, -1 past the path cap.  `calls` is checkLadderUseSearch's num_call at the end.
+template <int N>
+__device__ __forceinline__ int ladder_search(const TacPos& s0, int p, int16_t* path, int32_t* pend, const uint64_t* zob,
+                             const Lane& L, int& calls) {
+  const int victim = s0.meta.next, capturer = S_BLACK + S_WHITE - victim;
+  TacPos s = s0;
+  tac_play<N>(s, p, zob, L);
+  if (L.lane == 0) path[0] = (int16_t)p;
+  int len = 1, npend = 0;
+  calls = 0;
+  while (true) {
+    ++calls;
+    const uint32_t vic = victim == S_BLACK ? s.b : s.w;
+    const int lx = s.meta.last1 % N, ly = s.meta.last1 / N;
+    int next = -1;  // the child's move; -1: this node returns 0
+    bool played = false;
+    if (s.meta.next == capturer) {
+      // capturer to play: caught with one liberty, escaped with three or more
+      if (bit_at<N>(s.atari, lx, ly)) return len;
+      const uint32_t e = ~(s.b | s.w) & L.rm;
+      if (group_libs<N>(vic, e, lx, ly, L) == 2) {
+        const unsigned ed = empty_dirs<N>(e, lx, ly);
+        if (__popc(ed) == 2) {  // two liberties, both next to the last stone
+          const int esc0 = step4<N>(s.meta.last1, __ffs(ed) - 1), esc1 = step4<N>(s.meta.last1, __ffs(ed & (ed - 1)) - 1);
+          int must = -1;  // the first escape with three empty neighbours
+          if (__popc(empty_dirs<N>(e, esc0 % N, esc0 / N)) == 3)
+            must = esc0;
+          else if (__popc(empty_dirs<N>(e, esc1 % N, esc1 / N)) == 3)
+            must = esc1;
+          if (must < 0 && calls >= LADDER_BUDGET) must = esc0;  // too many branches: stop branching
+          if (must >= 0) {
+            if (tac_legal<N>(s, must, L)) next = must;
+          } else if (tac_legal<N>(s, esc0, L)) {
+            if (L.lane == 0) pend[npend] = (len << 16) | esc1;
+            ++npend;
+            next = esc0;
+          } else if (tac_legal<N>(s, esc1, L)) {
+            next = esc1;
+          }
+        }
+      }
+    } else if (!bit_at<N>(s.atari, lx, ly)) {
+      // victim to play, the capturer's last stone not in atari: flee to the first empty neighbour of the
+      // victim's last stone.  One always exists (the reference's "isLadderUseSearch is wrong" error is
+      // unreachable): the capturer node continued only with two empty escapes next to that stone and the
+      // capturer filled one of them.
+      const uint32_t e = ~(s.b | s.w) & L.rm;
+      const unsigned fd = empty_dirs<N>(e, s.meta.last2 % N, s.meta.last2 / N);
+      const int flee = step4<N>(s.meta.last2, __ffs(fd) - 1);
+      if (fd != 0u && tac_legal<N>(s, flee, L)) {
+        tac_play<N>(s, flee, zob, L);
+        played = true;
+        const int fx = flee % N, fy = flee / N;
+        const uint32_t e2 = ~(s.b | s.w) & L.rm;
+        const uint32_t vic2 = victim == S_BLACK ? s.b : s.w, cap2 = victim == S_BLACK ? s.w : s.b;
+        const int lib = group_libs<N>(vic2, e2, fx, fy, L);
+        bool escaped = lib >= 3;
+        if (lib == 2)  // two liberties and a capturer stone next to the flee point in atari: not a ladder
+          for (int d = 0; d < 4; ++d) escaped |= bit_at<N>(cap2 & s.atari, fx + d4x(d), fy + d4y(d));
+        if (!escaped) next = flee;
+      }
+    }
+    __syncwarp();
+    while (next < 0) {  // this node returns 0: back to the deepest pending branch and its escape[1]
+      if (npend == 0) return 0;
+      const int32_t pe = pend[--npend];
+      len = pe >> 16;
+      s = s0;
+      for (int i = 0; i < len; ++i) tac_play<N>(s, path[i], zob, L);
+      played = false;
+      if (tac_legal<N>(s, pe & 0xFFFF, L)) next = pe & 0xFFFF;
+    }
+    if (len == Tac<N>::MAX_PATH) return -1;
+    if (!played) tac_play<N>(s, next, zob, L);
+    if (L.lane == 0) path[len] = (int16_t)next;
+    ++len;
+    __syncwarp();
+  }
+}
+
+template <int N>
+__global__ void __launch_bounds__(TACTICS_WARPS * 32)
+    k_tactics(DevState st, int16_t* __restrict__ ladder, int16_t* __restrict__ self_atari,
+              int32_t* __restrict__ calls) {
+  constexpr int P = Geo<N>::P;
+  __shared__ uint64_t s_zob[Geo<N>::ZOB];
+  __shared__ int16_t s_path[TACTICS_WARPS][Tac<N>::MAX_PATH];
+  __shared__ int32_t s_pend[TACTICS_WARPS][Tac<N>::MAX_PEND];
+  load_zobrist<N>(s_zob);
+  const Lane L = make_lane_single<N>();
+  const int wid = threadIdx.x >> 5;
+  const int g = blockIdx.x * TACTICS_WARPS + wid;
+  if (g >= st.G) return;  // the whole warp
+  TacPos s0;
+  load_row<N>(st.cur, g, L.row, L.active, s0.b, s0.w);
+  load_row<N>(st.sa, g, L.row, L.active, s0.safe, s0.atari);
+  s0.meta = load_meta(&st.meta[g]);
+  s0.hash = st.hash[g];
+  const uint32_t e = ~(s0.b | s0.w) & L.rm;
+  // empty neighbours of every point: at least two / at least three of the four
+  const uint32_t el = (e << 1) & L.rm, er = e >> 1, eu = up_of<N>(e, L), ed = dn_of<N>(e, L);
+  const uint32_t ge2 = (el & er) | (eu & ed) | ((el | er) & (eu | ed));
+  const uint32_t ge3 = (el & er & (eu | ed)) | (eu & ed & (el | er));
+  const bool do_ladder = ladder || calls;
+  for (int ci = 0; ci < 2; ++ci) {
+    const int c = S_BLACK + ci;
+    const uint32_t own = c == S_BLACK ? s0.b : s0.w, opp = c == S_BLACK ? s0.w : s0.b;
+    const bool ko = (s0.meta.flags & F_KO_ACTIVE) && s0.meta.ko_color == c;
+    const uint32_t legal = legal_rows_cached<N>(own, opp, s0.safe, s0.atari, L, ko, s0.meta.ko_pt);
+    const size_t base = ((size_t)g * 2 + ci) * P + L.row;  // + x*N: this lane's point (x, row)
+    if (do_ladder) {
+      if (L.active)
+        for (int x = 0; x < N; ++x) {
+          if (ladder) ladder[base + x * N] = 0;
+          if (calls) calls[base + x * N] = 0;
+        }
+      uint32_t cand = legal & ge2 & ~ge3 & nbr4<N>(own & s0.atari, L) & nbr4<N>(opp, L);
+      while (__any_sync(FULL, cand != 0u)) {
+        const int y = __ffs(__ballot_sync(FULL, cand != 0u)) - 1;
+        const int x = __shfl_sync(FULL, __ffs(cand) - 1, y);
+        if (L.row == y) cand &= cand - 1;
+        int ex = -1, ey = -1;  // the enemy neighbour
+        for (int d = 0; d < 4; ++d)
+          if (ex < 0 && bit_at<N>(opp, x + d4x(d), y + d4y(d))) ex = x + d4x(d), ey = y + d4y(d);
+        if (group_libs<N>(opp, e, ex, ey, L) < 3) continue;
+        TacPos sc = s0;
+        sc.meta.next = (uint8_t)c;
+        int ncalls;
+        const int depth = ladder_search<N>(sc, y * N + x, s_path[wid], s_pend[wid], s_zob, L, ncalls);
+        if (L.active && L.row == y) {
+          if (ladder) ladder[base + x * N] = (int16_t)depth;
+          if (calls) calls[base + x * N] = ncalls;
+        }
+      }
+    }
+    if (self_atari) {
+      if (L.active)
+        for (int x = 0; x < N; ++x) self_atari[base + x * N] = 0;
+      uint32_t cand = legal & ~ge2;
+      while (__any_sync(FULL, cand != 0u)) {
+        const int y = __ffs(__ballot_sync(FULL, cand != 0u)) - 1;
+        const int x = __shfl_sync(FULL, __ffs(cand) - 1, y);
+        if (L.row == y) cand &= cand - 1;
+        const uint32_t me = (L.active && L.row == y) ? (1u << x) : 0u;
+        const uint32_t nb = nbr4<N>(me, L) & L.rm;
+        uint32_t grp[2] = {me | (nb & own), nb & opp & s0.atari};  // the new group; the groups it captures
+        const uint32_t thr[2] = {own | me, opp};
+        floodK<N, 2>(grp, thr, L);
+        const int libs = warp_rows_sum(__popc(nbr4<N>(grp[0], L) & ((e & ~me) | grp[1])), L);
+        const int stones = warp_rows_sum(__popc(grp[0]), L);
+        if (libs == 1 && L.active && L.row == y) self_atari[base + x * N] = (int16_t)stones;
+      }
+    }
+  }
+}
+
 }  // namespace elfb200
 
 // =========================================================================================
@@ -1102,7 +1349,8 @@ void elfb200_destroy(elfb200_ctx* c) {
                   c->st.sk_n, c->d_actions, c->d_ok,   c->d_bytes,   c->d_words,   c->d_d4,
                   c->d_feat,  c->d_po_sk, c->d_po_chk, c->d_po_hash, c->d_po_plies, c->d_po_score,
                   c->d_replay, c->st.placed, c->st.sa, c->d_exp_table, c->d_done,
-                  c->d_own_sk, c->d_own_counts, c->d_own_status, c->d_own_hash, c->d_own_plies};
+                  c->d_own_sk, c->d_own_counts, c->d_own_status, c->d_own_hash, c->d_own_plies,
+                  c->d_tac};
   for (void* p : ptrs)
     if (p) cudaFree(p);
   if (c->h_pin) cudaFreeHost(c->h_pin);
@@ -1713,6 +1961,47 @@ int elfb200_final_status(elfb200_ctx* c, const int32_t* counts_host, int playout
   if (dead_host) CK(cudaMemcpyAsync(dead_host, ddead, G * P, cudaMemcpyDeviceToHost, c->stream));
   if (territory_host) CK(cudaMemcpyAsync(territory_host, dterr, G * P, cudaMemcpyDeviceToHost, c->stream));
   if (score_host) CK(cudaMemcpyAsync(score_host, c->d_words, G * sizeof(int32_t), cudaMemcpyDeviceToHost, c->stream));
+  CK(cudaStreamSynchronize(c->stream));
+  return ELFB200_OK;
+}
+
+}  // extern "C"
+
+// ---- ladders and self-ataris -------------------------------------------------------------------------------------
+static int tactics_launch(elfb200_ctx* c, int16_t* ladder, int16_t* self_atari, int32_t* calls) {
+  const int grid = (c->G + TACTICS_WARPS - 1) / TACTICS_WARPS;
+  DISPATCH_N(c, (k_tactics<19><<<grid, TACTICS_WARPS * 32, 0, c->stream>>>(c->st, ladder, self_atari, calls)),
+             (k_tactics<9><<<grid, TACTICS_WARPS * 32, 0, c->stream>>>(c->st, ladder, self_atari, calls)));
+  c->launches++;
+  CK(cudaGetLastError());
+  return ELFB200_OK;
+}
+
+extern "C" {
+
+int elfb200_tactics_dev(elfb200_ctx* c, int16_t* ladder_dev, int16_t* self_atari_dev) {
+  if (!c) return elfb200_fail(ELFB200_ERR_ARG, "ctx is NULL");
+  if (((uintptr_t)ladder_dev | (uintptr_t)self_atari_dev) & 1u)
+    return elfb200_fail(ELFB200_ERR_ARG, "ladder / self_atari must be 2-byte aligned");
+  if (!ladder_dev && !self_atari_dev) return ELFB200_OK;
+  CK(cudaSetDevice(c->device));
+  return tactics_launch(c, ladder_dev, self_atari_dev, nullptr);
+}
+
+int elfb200_tactics(elfb200_ctx* c, int16_t* ladder_host, int16_t* self_atari_host, int32_t* calls_host) {
+  if (!c) return elfb200_fail(ELFB200_ERR_ARG, "ctx is NULL");
+  if (!ladder_host && !self_atari_host && !calls_host) return ELFB200_OK;
+  CK(cudaSetDevice(c->device));
+  const size_t n = (size_t)c->G * 2 * c->N * c->N;
+  if (!c->d_tac) CK(cudaMalloc(&c->d_tac, n * (2 * sizeof(int16_t) + sizeof(int32_t))));
+  int16_t* dl = ladder_host ? (int16_t*)c->d_tac : nullptr;
+  int16_t* ds = self_atari_host ? (int16_t*)c->d_tac + n : nullptr;
+  int32_t* dc = calls_host ? (int32_t*)((int16_t*)c->d_tac + 2 * n) : nullptr;
+  int rc = tactics_launch(c, dl, ds, dc);
+  if (rc) return rc;
+  if (dl) CK(cudaMemcpyAsync(ladder_host, dl, n * sizeof(int16_t), cudaMemcpyDeviceToHost, c->stream));
+  if (ds) CK(cudaMemcpyAsync(self_atari_host, ds, n * sizeof(int16_t), cudaMemcpyDeviceToHost, c->stream));
+  if (dc) CK(cudaMemcpyAsync(calls_host, dc, n * sizeof(int32_t), cudaMemcpyDeviceToHost, c->stream));
   CK(cudaStreamSynchronize(c->stream));
   return ELFB200_OK;
 }

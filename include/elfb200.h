@@ -197,6 +197,22 @@ int elfb200_ownership_dev(elfb200_ctx* ctx, int playouts, uint64_t seed, int max
 int elfb200_final_status(elfb200_ctx* ctx, const int32_t* counts_host, int playouts, double threshold,
                          uint8_t* dead_host, uint8_t* territory_host, int32_t* score_host);
 
+/* Ladders and self-ataris of the stored positions, for every point and both colours whoever is to move (colour
+ * index 0 = black, 1 = white), by action x*N+y, int16 [G][2][N*N] each.  With ids = TryPlay(board, x, y, c, &ids)
+ * (board.cc:788-827; both values are 0 where it refuses the move):
+ *   ladder      checkLadder(board, &ids, c) (board.cc:476-524, search checkLadderUseSearch board.cc:299-439): the
+ *               depth at which c's group, escaping by this move, is caught; 0 when it is not a ladder.  -1 marks a
+ *               search longer than 2*N*N plies, which this library does not follow; the reference never returns it.
+ *   self_atari  isSelfAtari(board, &ids, c, c, &num_stones) (board.cc:242-297): num_stones when it is true (the
+ *               stones of the group the move leaves with one liberty), else 0.
+ * calls int32 [G][2][N*N]: checkLadderUseSearch's num_call for each search (0 where none ran; the budget
+ * MAX_LADDER_SEARCH = 1024 stops its branching).  Any output may be NULL and its work is skipped.  The stored
+ * games are not changed.  Synchronous. */
+int elfb200_tactics(elfb200_ctx* ctx, int16_t* ladder_host, int16_t* self_atari_host, int32_t* calls_host);
+/* The same ladder / self_atari into device memory (either may be NULL; 2-byte aligned), asynchronous on the context
+ * stream.  Needs no scratch: capturable in a CUDA graph from the first call. */
+int elfb200_tactics_dev(elfb200_ctx* ctx, int16_t* ladder_dev, int16_t* self_atari_dev);
+
 /* Number of kernels this library has launched since creation (bench gpu_launches).  Counts enqueues by
  * the calls above; replays of a CUDA graph that captured them are not counted. */
 int64_t elfb200_launch_count(const elfb200_ctx* ctx);
