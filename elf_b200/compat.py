@@ -351,6 +351,7 @@ class SelfPlayEngine:
         self.sp = selfplay
         self.board_size = selfplay.N
         self.num_action = selfplay.N * selfplay.N + 1
+        self.num_planes = 25 if getattr(selfplay, "use_df_feature", False) else 18
         self.resign_thres = selfplay.resign_thres
         import collections
 
@@ -522,6 +523,7 @@ class OnlineEngine:
         self.game = game
         self.board_size = game.N
         self.num_action = game.N * game.N + 1
+        self.num_planes = 25 if getattr(game, "use_df_feature", False) else 18
         self._gen = None
         self._wave = None
         self.last_status = None
@@ -559,7 +561,8 @@ class OnlineEngine:
         import torch
 
         if self._gen is None:
-            return 1, torch.from_numpy(self.game.board.features())
+            b = self.game.board
+            return 1, torch.from_numpy(b.features_df() if self.num_planes == 25 else b.features())
         w = self._wave
         if w["off"] >= w["n"]:
             raise RuntimeError("wait() called again before step() answered the previous batch")
@@ -762,6 +765,8 @@ def game_context(co, opt, board_size=19, device=0, factories=None):
             # GameOptions::seed != 0: every game thread's generator starts from it (game_base.h:32-38) and
             # the reference's games are reproducible -- ours are then the same games (elf_b200.refstream)
             kw["rng"] = "reference"
+        if bool(getattr(opt, "use_df_feature", False)):
+            kw["use_df_feature"] = True
         sp = f.get("selfplay", SelfPlay)(**kw)
         return GameContext(SelfPlayEngine(sp), batchsize=int(co.batchsize))
     if opt.mode == "online":
@@ -771,6 +776,8 @@ def game_context(co, opt, board_size=19, device=0, factories=None):
                   policy_distri_cutoff=int(opt.policy_distri_cutoff), move_cutoff=int(opt.move_cutoff),
                   preload_sgf=opt.preload_sgf or None, preload_sgf_move_to=int(opt.preload_sgf_move_to),
                   following_pass=bool(opt.following_pass), seed=int(opt.seed), **{k: v for k, v in common.items() if k != "komi"})
+        if bool(getattr(opt, "use_df_feature", False)):
+            kw["use_df_feature"] = True
         game = f.get("online", OnlineGame.create)(**kw)
         return GameContext(OnlineEngine(game), batchsize=int(co.batchsize))
     if opt.mode in ("train", "offline_train"):

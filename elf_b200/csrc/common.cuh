@@ -97,7 +97,10 @@ __device__ __forceinline__ void d4_inverse(int N, int d4, int tx, int ty, int& x
 // channels-last convolutions: [n][N][N][cpad] with the 18 planes in channels 0..17 and zeros above
 // (cpad a multiple of 8: 16 bytes per 8 channels), so the network's input cast/permute pass
 // disappears.  Values are exactly 0.0 / 1.0 in every format.
-enum : int { FEAT_F32_NCHW = 0, FEAT_F16_NHWC = 1, FEAT_BF16_NHWC = 2 };
+// FEAT_DF_F32_NCHW is the other plane set of the GoFeature contract: the 25 DarkForest planes of
+// BoardFeature::extract (GameOptions::use_df_feature, game_feature.h:22-33), float32 [n][25][N][N];
+// written by df_planes below, not by features_cta.
+enum : int { FEAT_F32_NCHW = 0, FEAT_F16_NHWC = 1, FEAT_BF16_NHWC = 2, FEAT_DF_F32_NCHW = 3 };
 
 // Shared -> global bulk copy (TMA engine, `cp.async.bulk`): one thread hands the whole staged tile
 // to the copy engine instead of every thread issuing stores.  `bytes` a multiple of 16, both
@@ -321,6 +324,103 @@ __device__ __forceinline__ void features_cta(Gather gather, int n_pos, void* __r
       *reinterpret_cast<float2*>(dst + b0) = make_float2((w & 1u) ? 1.0f : 0.0f, (w & 2u) ? 1.0f : 0.0f);
     }
   }
+}
+
+// ---- DarkForest planes ----------------------------------------------------------------------------
+// BoardFeature::extract (board_feature.cc:209-237): the 25-plane DarkForest feature set of one position,
+// float32 [25][N][N] under a D4 code.  Filled planes (board_feature.h:19-36): 0-2 our groups with
+// 1 / 2 / >=3 liberties, 3-5 the opponent's, 6 the simple-ko point, 7 / 8 / 9 our / opponent / empty
+// points, 10 / 11 exp((last_placed - ply) / 10) on our / the opponent's stones, 14 / 15 the L1 distance
+// to the nearest stone of ours / theirs (10000 if there is none), 16 / 17 black / white to move; the
+// other planes stay zero.  One warp = one position (row per lane): `b` / `w` are the lane's board row,
+// `placed` (shared memory, N*N) the ply each stone was placed at, `exp_tab[k]` = exp(-k/10) from the host's
+// libm.  The planes are staged in `tile` (shared, 25*N*N floats) in OUTPUT order (cell = Transform(x, y),
+// board_feature.h:97-113) and leave coalesced to `dst`.  Both the board batch (k_features_df) and the
+// search's leaf batch (k_leaf_features_df) write their planes through this function.
+template <int N>
+__device__ __forceinline__ void df_planes(const Lane& L, uint32_t b, uint32_t w, const BoardMeta& meta, int d4,
+                                          const uint16_t* placed, const float* __restrict__ exp_tab, float* tile,
+                                          uint8_t (*hd)[N], float* __restrict__ dst) {
+  constexpr int P = Geo<N>::P;
+  const bool bf = meta.next == S_BLACK;
+  const uint32_t own = bf ? b : w, opp = bf ? w : b;
+  const uint32_t e = ~(own | opp) & L.rm;
+  for (int i = L.lane; i < 25 * P; i += 32) tile[i] = 0.f;
+  __syncwarp();
+  auto cell = [&](int x, int y) -> int {  // Transform: rotate, then flip
+    int ta, tb;
+    switch (d4 & 3) {
+      case 1: ta = y; tb = N - 1 - x; break;
+      case 2: ta = N - 1 - x; tb = N - 1 - y; break;
+      case 3: ta = N - 1 - y; tb = x; break;
+      default: ta = x; tb = y; break;
+    }
+    return (d4 & 4) ? tb * N + ta : ta * N + tb;
+  };
+  if (L.active) {
+    for (int x = 0; x < N; ++x) {
+      const int c = cell(x, L.row);
+      const bool ob = (own >> x) & 1u, pb = (opp >> x) & 1u;
+      tile[7 * P + c] = ob ? 1.f : 0.f;
+      tile[8 * P + c] = pb ? 1.f : 0.f;
+      tile[9 * P + c] = (ob || pb) ? 0.f : 1.f;
+      if (ob || pb) tile[(ob ? 10 : 11) * P + c] = exp_tab[(int)meta.ply - (int)placed[L.row * N + x]];
+      tile[(bf ? 16 : 17) * P + c] = 1.f;
+    }
+  }
+  if (L.lane == 0 && (meta.flags & F_KO_ACTIVE) && meta.ko_pt >= 0)  // getSimpleKoLocation, board.cc:466-474
+    tile[6 * P + cell(meta.ko_pt % N, meta.ko_pt / N)] = 1.f;
+  // liberty classes, group by group (getLibertyMap3binary, board_feature.cc:93-113)
+  {
+    const Links k = make_links<N>(own, opp, L);
+    uint32_t todo = own | opp;
+    while (__any_sync(FULL, todo != 0u)) {
+      const uint32_t bal = __ballot_sync(FULL, todo != 0u);
+      const int src = __ffs(bal) - 1;
+      uint32_t grp = (L.lane == src) ? (todo & (0u - todo)) : 0u;
+      while (true) {
+        const uint32_t g1 = grow_link(grp, k);
+        const uint32_t g2 = grow_link(g1, k);
+        const bool ch = g2 != grp;
+        grp = g2;
+        if (!__any_sync(FULL, ch)) break;
+      }
+      const int nl = __reduce_add_sync(FULL, __popc(nbr4<N>(grp, L) & e));
+      const bool ours = __any_sync(FULL, (grp & own) != 0u);
+      const int plane = (ours ? 0 : 3) + (nl == 1 ? 0 : nl == 2 ? 1 : 2);
+      for (uint32_t m = grp; m; m &= m - 1) tile[plane * P + cell(__ffs(m) - 1, L.row)] = 1.f;
+      todo &= ~grp;
+    }
+  }
+  // distance to the nearest stone of each colour (getDistanceMap + DistanceTransform, board_feature.cc:20-40,
+  // 181-196): the two 1-D min-plus sweeps there are the exact L1 distance transform, which commutes with D4
+  for (int side = 0; side < 2; ++side) {
+    const uint32_t row = side == 0 ? own : opp;
+    __syncwarp();
+    if (L.active) {
+      for (int x = 0; x < N; ++x) {
+        int d = 255;
+        const uint32_t lo = row & ((2u << x) - 1u), hi = row >> x;
+        if (lo) d = x - (31 - __clz(lo));
+        if (hi) d = min(d, __ffs(hi) - 1);
+        hd[L.row][x] = (uint8_t)d;
+      }
+    }
+    __syncwarp();
+    const bool none = !__any_sync(FULL, row != 0u);
+    if (L.active) {
+      for (int x = 0; x < N; ++x) {
+        int best = 100000;
+        for (int y2 = 0; y2 < N; ++y2) {
+          const int h = hd[y2][x];
+          if (h != 255) best = min(best, h + (y2 > L.row ? y2 - L.row : L.row - y2));
+        }
+        tile[(14 + side) * P + cell(x, L.row)] = none ? 10000.f : (float)best;
+      }
+    }
+  }
+  __syncwarp();
+  for (int i = L.lane; i < 25 * P; i += 32) dst[i] = tile[i];
 }
 
 template <int N>

@@ -498,14 +498,11 @@ __global__ void __launch_bounds__(FEAT_THREADS)
 }
 
 // ---------------------------------------------------------------------------------------
-// BoardFeature::extract (board_feature.cc:209-237): the 25-plane DarkForest feature set
-// (GameOptions::use_df_feature), float32 [G][25][N][N] under a D4 code.  Filled planes (board_feature.h:19-36):
-// 0-2 our groups with 1 / 2 / >=3 liberties, 3-5 the opponent's, 6 the simple-ko point, 7 / 8 / 9 our /
-// opponent / empty points, 10 / 11 exp((last_placed - ply) / 10) on our / the opponent's stones, 14 / 15 the
-// L1 distance to the nearest stone of ours / theirs (10000 if there is none), 16 / 17 black / white to move;
-// the other planes stay zero.  One warp = one game (row per lane); the planes are staged in shared
-// memory in OUTPUT order (cell = Transform(x, y), board_feature.h:97-113) and leave coalesced.
-// Not on the self-play hot path (AGZ features are); built for parity of the offline/DF path.
+// BoardFeature::extract (board_feature.cc:209-237) for the board batch: the 25-plane DarkForest feature
+// set (GameOptions::use_df_feature), float32 [G][25][N][N] under a D4 code; the planes are df_planes'
+// (common.cuh), which the search's leaf writer k_leaf_features_df shares.  One warp = one game.
+// Used by training replay and the online human_actor position; the search writes its leaves with
+// k_leaf_features_df.
 template <int N>
 __global__ void __launch_bounds__(32)
     k_features_df(DevState st, const int32_t* __restrict__ d4codes, const float* __restrict__ exp_tab,
@@ -513,6 +510,7 @@ __global__ void __launch_bounds__(32)
   constexpr int P = Geo<N>::P;
   __shared__ float tile[25 * P];
   __shared__ uint8_t hd[N][N];
+  __shared__ uint16_t placed[P];
   const Lane L = make_lane_single<N>();
   const int g = blockIdx.x;
   if (g >= st.G) return;
@@ -520,87 +518,9 @@ __global__ void __launch_bounds__(32)
   load_row<N>(st.cur, g, L.row, L.active, b, w);
   const BoardMeta meta = load_meta(&st.meta[g]);
   const int d4 = d4codes ? d4codes[g] : 0;
-  const bool bf = meta.next == S_BLACK;
-  const uint32_t own = bf ? b : w, opp = bf ? w : b;
-  const uint32_t e = ~(own | opp) & L.rm;
-  for (int i = L.lane; i < 25 * P; i += 32) tile[i] = 0.f;
+  for (int i = L.lane; i < P; i += 32) placed[i] = st.placed[(size_t)g * P + i];
   __syncwarp();
-  auto cell = [&](int x, int y) -> int {  // Transform: rotate, then flip
-    int ta, tb;
-    switch (d4 & 3) {
-      case 1: ta = y; tb = N - 1 - x; break;
-      case 2: ta = N - 1 - x; tb = N - 1 - y; break;
-      case 3: ta = N - 1 - y; tb = x; break;
-      default: ta = x; tb = y; break;
-    }
-    return (d4 & 4) ? tb * N + ta : ta * N + tb;
-  };
-  const uint16_t* placed = st.placed + (size_t)g * P;
-  if (L.active) {
-    for (int x = 0; x < N; ++x) {
-      const int c = cell(x, L.row);
-      const bool ob = (own >> x) & 1u, pb = (opp >> x) & 1u;
-      tile[7 * P + c] = ob ? 1.f : 0.f;
-      tile[8 * P + c] = pb ? 1.f : 0.f;
-      tile[9 * P + c] = (ob || pb) ? 0.f : 1.f;
-      if (ob || pb) tile[(ob ? 10 : 11) * P + c] = exp_tab[(int)meta.ply - (int)placed[L.row * N + x]];
-      tile[(bf ? 16 : 17) * P + c] = 1.f;
-    }
-  }
-  if (L.lane == 0 && (meta.flags & F_KO_ACTIVE) && meta.ko_pt >= 0)  // getSimpleKoLocation, board.cc:466-474
-    tile[6 * P + cell(meta.ko_pt % N, meta.ko_pt / N)] = 1.f;
-  // liberty classes, group by group (getLibertyMap3binary, board_feature.cc:93-113)
-  {
-    const Links k = make_links<N>(own, opp, L);
-    uint32_t todo = own | opp;
-    while (__any_sync(FULL, todo != 0u)) {
-      const uint32_t bal = __ballot_sync(FULL, todo != 0u);
-      const int src = __ffs(bal) - 1;
-      uint32_t grp = (L.lane == src) ? (todo & (0u - todo)) : 0u;
-      while (true) {
-        const uint32_t g1 = grow_link(grp, k);
-        const uint32_t g2 = grow_link(g1, k);
-        const bool ch = g2 != grp;
-        grp = g2;
-        if (!__any_sync(FULL, ch)) break;
-      }
-      const int nl = __reduce_add_sync(FULL, __popc(nbr4<N>(grp, L) & e));
-      const bool ours = __any_sync(FULL, (grp & own) != 0u);
-      const int plane = (ours ? 0 : 3) + (nl == 1 ? 0 : nl == 2 ? 1 : 2);
-      for (uint32_t m = grp; m; m &= m - 1) tile[plane * P + cell(__ffs(m) - 1, L.row)] = 1.f;
-      todo &= ~grp;
-    }
-  }
-  // distance to the nearest stone of each colour (getDistanceMap + DistanceTransform, board_feature.cc:20-40,
-  // 181-196): the two 1-D min-plus sweeps there are the exact L1 distance transform, which commutes with D4
-  for (int side = 0; side < 2; ++side) {
-    const uint32_t row = side == 0 ? own : opp;
-    __syncwarp();
-    if (L.active) {
-      for (int x = 0; x < N; ++x) {
-        int d = 255;
-        const uint32_t lo = row & ((2u << x) - 1u), hi = row >> x;
-        if (lo) d = x - (31 - __clz(lo));
-        if (hi) d = min(d, __ffs(hi) - 1);
-        hd[L.row][x] = (uint8_t)d;
-      }
-    }
-    __syncwarp();
-    const bool none = !__any_sync(FULL, row != 0u);
-    if (L.active) {
-      for (int x = 0; x < N; ++x) {
-        int best = 100000;
-        for (int y2 = 0; y2 < N; ++y2) {
-          const int h = hd[y2][x];
-          if (h != 255) best = min(best, h + (y2 > L.row ? y2 - L.row : L.row - y2));
-        }
-        tile[(14 + side) * P + cell(x, L.row)] = none ? 10000.f : (float)best;
-      }
-    }
-  }
-  __syncwarp();
-  float* dst = out + (size_t)g * 25 * P;
-  for (int i = L.lane; i < 25 * P; i += 32) dst[i] = tile[i];
+  df_planes<N>(L, b, w, meta, d4, placed, exp_tab, tile, hd, out + (size_t)g * 25 * P);
 }
 
 // ---------------------------------------------------------------------------------------
@@ -1677,9 +1597,11 @@ int elfb200_evaluate(elfb200_ctx* c, float komi, float* value_host) {
 }
 
 static int check_feature_args(const void* out, int format, int cpad) {
-  if (format < FEAT_F32_NCHW || format > FEAT_BF16_NHWC) return elfb200_fail(ELFB200_ERR_ARG, "unknown feature format %d", format);
+  if (format < FEAT_F32_NCHW || format > FEAT_DF_F32_NCHW) return elfb200_fail(ELFB200_ERR_ARG, "unknown feature format %d", format);
   const uintptr_t a = (uintptr_t)out;
-  if (format == FEAT_F32_NCHW) {
+  if (format == FEAT_DF_F32_NCHW) {
+    if (a & 3) return elfb200_fail(ELFB200_ERR_ARG, "feature buffer must be 4-byte aligned");
+  } else if (format == FEAT_F32_NCHW) {
     if (a & 7) return elfb200_fail(ELFB200_ERR_ARG, "feature buffer must be 8-byte aligned");
   } else {
     if (cpad < 24 || cpad > FEAT_CPAD_MAX || (cpad & 7))
@@ -1693,6 +1615,7 @@ int elfb200_features_dev_ex(elfb200_ctx* c, const int32_t* d4_dev, void* out_dev
   if (!c || !out_dev) return elfb200_fail(ELFB200_ERR_ARG, "NULL argument");
   int rc = check_feature_args(out_dev, format, cpad);
   if (rc) return rc;
+  if (format == FEAT_DF_F32_NCHW) return elfb200_features_df_dev(c, d4_dev, static_cast<float*>(out_dev));  // cpad ignored
   CK(cudaSetDevice(c->device));
   DISPATCH_N(c,
              (k_features<19><<<c->G, FEAT_THREADS, feature_smem_bytes<19>(format, cpad, c->feat_tma), c->stream>>>(

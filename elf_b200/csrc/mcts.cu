@@ -24,7 +24,7 @@
 //
 // Kernels: k_begin (root set-up), k_select (PUCT descent + child state creation + terminal
 // evaluation + leaf claim), k_leaf_features (18-plane stack per claimed leaf, history gathered
-// along the parent chain), k_expand (mask/sort/renormalise the net's policy into edges),
+// along the parent chain; k_leaf_features_df: the 25 DarkForest planes instead), k_expand (mask/sort/renormalise the net's policy into edges),
 // k_backup, k_results, k_advance (tree reuse: keep the chosen child's subtree, free the rest).
 #include <cfloat>
 
@@ -696,6 +696,64 @@ template <int N>
 __global__ void __launch_bounds__(FEAT_THREADS)
     k_leaf_features(TreeDev tr, void* __restrict__ out, int fmt, int cpad, int tma) {
   features_cta<N>(StagedGather<N>{tr.hist, tr.hinfo}, *tr.eval_count, out, fmt, cpad, tma);
+}
+
+// ---------------------------------------------------------------------------------------
+// BoardFeature::extract (the 25 DarkForest planes, GameOptions::use_df_feature) for every claimed leaf, in
+// claim order and under the leaf's D4 code, so the rows line up with k_expand exactly as
+// k_leaf_features' do.  One warp per leaf; the planes are df_planes' (common.cuh), shared with the board
+// batch's k_features_df.
+//
+// Position and meta come from the leaf's node (not from hist: at a ply-1 root with handicap stones the
+// AGZ history is empty by design, the DF stone and liberty planes are not).  The DF history planes need
+// the ply every stone on the leaf's board was placed at (Info::last_placed).  The board batch holds the
+// root position during a move, so `placed` starts as the board's array; then every non-pass node on the
+// parent chain from the leaf up to (not including) the game's root placed a stone at meta.last1 at ply
+// meta.ply - 1 -- what k_step writes.  The move nearest the leaf wins at each point; a stone with no move
+// on the chain was on the board at the root.  Descents are at most MAX_DEPTH plies deep, which bounds the
+// chain.  Shared memory: the 25*N*N float tile plus N*N 16-bit plies, about 37 KB at 19x19.
+template <int N>
+__global__ void __launch_bounds__(32)
+    k_leaf_features_df(TreeDev tr, DevState st, const float* __restrict__ exp_tab, float* __restrict__ out) {
+  constexpr int P = Geo<N>::P;
+  __shared__ float tile[25 * P];
+  __shared__ uint8_t hd[N][N];
+  __shared__ uint16_t placed[P];
+  __shared__ uint16_t chain[MAX_DEPTH + 1];
+  __shared__ int16_t chain_pt[MAX_DEPTH + 1];
+  __shared__ uint16_t chain_ply[MAX_DEPTH + 1];
+  __shared__ int s_len;
+  const Lane L = make_lane_single<N>();
+  const int slot = blockIdx.x;
+  if (slot >= *tr.eval_count) return;
+  const int g = tr.eval_game[slot], node = tr.eval_node[slot], d4 = tr.eval_d4[slot];
+  const size_t nb = (size_t)g * tr.C;
+  const uint64_t rowv = L.active ? tr.pos[(nb + node) * N + L.row] : 0ull;
+  const BoardMeta meta = load_meta(&tr.meta[nb + node]);
+  for (int i = L.lane; i < P; i += 32) placed[i] = st.placed[(size_t)g * P + i];
+  if (L.lane == 0) {  // leaf -> root: a chain of dependent parent reads
+    const int root = tr.root[g];
+    int nd = node, len = 0;
+    while (nd != root && nd != NONE16 && len <= MAX_DEPTH) {
+      chain[len++] = (uint16_t)nd;
+      nd = tr.hdr[nb + nd].parent;
+    }
+    s_len = len;
+  }
+  __syncwarp();
+  const int len = s_len;
+  for (int i = L.lane; i < len; i += 32) {
+    const BoardMeta m = load_meta(&tr.meta[nb + chain[i]]);
+    chain_pt[i] = m.last1;
+    chain_ply[i] = (uint16_t)(m.ply - 1);
+  }
+  __syncwarp();
+  if (L.lane == 0)  // root side first, so the move nearest the leaf is written last
+    for (int i = len - 1; i >= 0; --i)
+      if (chain_pt[i] >= 0) placed[chain_pt[i]] = chain_ply[i];
+  __syncwarp();
+  df_planes<N>(L, (uint32_t)rowv, (uint32_t)(rowv >> 32), meta, d4, placed, exp_tab, tile, hd,
+               out + (size_t)slot * 25 * P);
 }
 
 // ---------------------------------------------------------------------------------------
@@ -1453,6 +1511,35 @@ static void flush_timings(elfb200_mcts* m) {  // caller has synchronised the str
 
 static inline int warp_grid(int G) { return (G + WARPS - 1) / WARPS; }
 
+// The leaf-batch formats (ELFB200_FEAT_*): the AGZ planes in float32 NCHW or 16-bit NHWC (cpad 24 / 32),
+// or the DarkForest planes in float32 NCHW (cpad ignored).
+static int check_leaf_format(const void* feat_dev, int format, int cpad) {
+  if (format < FEAT_F32_NCHW || format > FEAT_DF_F32_NCHW) return elfb200_fail(ELFB200_ERR_ARG, "unknown feature format %d", format);
+  if ((format == FEAT_F16_NHWC || format == FEAT_BF16_NHWC) && (cpad < 24 || cpad > FEAT_CPAD_MAX || (cpad & 7)))
+    return elfb200_fail(ELFB200_ERR_ARG, "channel padding must be 24 or 32 (got %d)", cpad);
+  if ((uintptr_t)feat_dev & 15) return elfb200_fail(ELFB200_ERR_ARG, "leaf feature buffer must be 16-byte aligned");
+  return ELFB200_OK;
+}
+
+// The planes of the claimed leaves: `npos` CTAs, the kernels stop at the device-side count.
+static void launch_leaf_features(elfb200_mcts* m, void* feat_dev, int format, int cpad, int npos) {
+  elfb200_ctx* c = m->ctx;
+  if (format == FEAT_DF_F32_NCHW) {
+    DISPATCH_N(c,
+               (k_leaf_features_df<19><<<npos, 32, 0, c->stream>>>(m->tr, c->st, c->d_exp_table,
+                                                                   static_cast<float*>(feat_dev))),
+               (k_leaf_features_df<9><<<npos, 32, 0, c->stream>>>(m->tr, c->st, c->d_exp_table,
+                                                                  static_cast<float*>(feat_dev))));
+  } else {
+    DISPATCH_N(c,
+               (k_leaf_features<19><<<npos, FEAT_THREADS, feature_smem_bytes<19>(format, cpad, c->feat_tma), c->stream>>>(
+                   m->tr, feat_dev, format, cpad, c->feat_tma)),
+               (k_leaf_features<9><<<npos, FEAT_THREADS, feature_smem_bytes<9>(format, cpad, c->feat_tma), c->stream>>>(
+                   m->tr, feat_dev, format, cpad, c->feat_tma)));
+  }
+  c->launches++;
+}
+
 extern "C" {
 
 int elfb200_mcts_default_options(elfb200_mcts_options* o) {
@@ -1637,10 +1724,8 @@ int elfb200_mcts_begin_move(elfb200_mcts* m, const uint8_t* active_host) {
 int elfb200_mcts_select_ex(elfb200_mcts* m, void* feat_dev, int format, int cpad, int32_t* n_leaves) {
   if (!m || !feat_dev) return elfb200_fail(ELFB200_ERR_ARG, "NULL argument");
   elfb200_ctx* c = m->ctx;
-  if (format < FEAT_F32_NCHW || format > FEAT_BF16_NHWC) return elfb200_fail(ELFB200_ERR_ARG, "unknown feature format %d", format);
-  if (format != FEAT_F32_NCHW && (cpad < 24 || cpad > FEAT_CPAD_MAX || (cpad & 7)))
-    return elfb200_fail(ELFB200_ERR_ARG, "channel padding must be 24 or 32 (got %d)", cpad);
-  if ((uintptr_t)feat_dev & 15) return elfb200_fail(ELFB200_ERR_ARG, "leaf feature buffer must be 16-byte aligned");
+  const int rc = check_leaf_format(feat_dev, format, cpad);
+  if (rc) return rc;
   CK(cudaSetDevice(c->device));
   if (m->pending_sel || m->pending_feat || m->pending_eb) {
     // the event pairs are reused every wave: read the previous wave's before re-recording them
@@ -1673,12 +1758,7 @@ int elfb200_mcts_select_ex(elfb200_mcts* m, void* feat_dev, int format, int cpad
   if (n != 0) {
     const int npos = n > 0 ? n : c->G * m->tr.B;
     CK(cudaEventRecord(m->ev[2], c->stream));
-    DISPATCH_N(c,
-               (k_leaf_features<19><<<npos, FEAT_THREADS, feature_smem_bytes<19>(format, cpad, c->feat_tma), c->stream>>>(
-                   m->tr, feat_dev, format, cpad, c->feat_tma)),
-               (k_leaf_features<9><<<npos, FEAT_THREADS, feature_smem_bytes<9>(format, cpad, c->feat_tma), c->stream>>>(
-                   m->tr, feat_dev, format, cpad, c->feat_tma)));
-    c->launches++;
+    launch_leaf_features(m, feat_dev, format, cpad, npos);
     CK(cudaGetLastError());
     CK(cudaEventRecord(m->ev[3], c->stream));
     m->pending_feat = true;
@@ -1690,20 +1770,13 @@ int elfb200_mcts_select_ex(elfb200_mcts* m, void* feat_dev, int format, int cpad
 int elfb200_mcts_leaf_features(elfb200_mcts* m, void* feat_dev, int format, int cpad) {
   if (!m || !feat_dev) return elfb200_fail(ELFB200_ERR_ARG, "NULL argument");
   elfb200_ctx* c = m->ctx;
-  if (format < FEAT_F32_NCHW || format > FEAT_BF16_NHWC) return elfb200_fail(ELFB200_ERR_ARG, "unknown feature format %d", format);
-  if (format != FEAT_F32_NCHW && (cpad < 24 || cpad > FEAT_CPAD_MAX || (cpad & 7)))
-    return elfb200_fail(ELFB200_ERR_ARG, "channel padding must be 24 or 32 (got %d)", cpad);
-  if ((uintptr_t)feat_dev & 15) return elfb200_fail(ELFB200_ERR_ARG, "leaf feature buffer must be 16-byte aligned");
+  const int rc = check_leaf_format(feat_dev, format, cpad);
+  if (rc) return rc;
   CK(cudaSetDevice(c->device));
   const int n = m->last_eval_count;
   if (n == 0) return ELFB200_OK;
   const int npos = n > 0 ? n : c->G * m->tr.B;
-  DISPATCH_N(c,
-             (k_leaf_features<19><<<npos, FEAT_THREADS, feature_smem_bytes<19>(format, cpad, c->feat_tma), c->stream>>>(
-                 m->tr, feat_dev, format, cpad, c->feat_tma)),
-             (k_leaf_features<9><<<npos, FEAT_THREADS, feature_smem_bytes<9>(format, cpad, c->feat_tma), c->stream>>>(
-                 m->tr, feat_dev, format, cpad, c->feat_tma)));
-  c->launches++;
+  launch_leaf_features(m, feat_dev, format, cpad, npos);
   CK(cudaGetLastError());
   return ELFB200_OK;
 }

@@ -20,7 +20,7 @@ import torch
 from . import lib as _l
 from .board import GoBatch
 
-_FORMATS = {"f32": _l.FEAT_F32_NCHW, "f16": _l.FEAT_F16_NHWC, "bf16": _l.FEAT_BF16_NHWC}
+_FORMATS = {"f32": _l.FEAT_F32_NCHW, "f16": _l.FEAT_F16_NHWC, "bf16": _l.FEAT_BF16_NHWC, "df": _l.FEAT_DF_F32_NCHW}
 
 
 def random_legal_actions(legal, counter, seed=0):
@@ -45,7 +45,8 @@ def random_legal_actions(legal, counter, seed=0):
 class GoEnv:
     """``board``: a :class:`GoBatch` (or an object with its ``_lib`` / ``_ctx`` / ``num_games`` /
     ``board_size`` / ``device`` / ``stream`` attributes).  ``features``: None (no planes), ``"f32"``
-    (float32 ``[G,18,N,N]``) or ``"f16"`` / ``"bf16"`` (``[G,N,N,cpad]`` channels-last).  ``device``: where
+    (float32 ``[G,18,N,N]``), ``"f16"`` / ``"bf16"`` (``[G,N,N,cpad]`` channels-last) or ``"df"`` (the 25
+    DarkForest planes of ``GameOptions::use_df_feature``, float32 ``[G,25,N,N]``).  ``device``: where
     the observation tensors live, by default the board's CUDA device; a board whose kernels run on the host
     (the SIMT emulator build used by the tests) takes ``"cpu"``, and then no stream work is done.
 
@@ -56,7 +57,7 @@ class GoEnv:
 
     def __init__(self, board, komi=7.5, features=None, cpad=24, device=None):
         if features is not None and features not in _FORMATS:
-            raise ValueError("features must be None, 'f32', 'f16' or 'bf16'")
+            raise ValueError("features must be None, 'f32', 'f16', 'bf16' or 'df'")
         self.board = board
         self._lib, self._ctx = board._lib, board._ctx
         G, n = board.num_games, board.board_size
@@ -75,8 +76,8 @@ class GoEnv:
         self._fmt = _FORMATS.get(features)
         if features is None:
             self.planes = None
-        elif features == "f32":
-            self.planes = torch.zeros((G, 18, n, n), dtype=torch.float32, device=dev)
+        elif features in ("f32", "df"):
+            self.planes = torch.zeros((G, 18 if features == "f32" else 25, n, n), dtype=torch.float32, device=dev)
         else:
             dt = torch.float16 if features == "f16" else torch.bfloat16
             self.planes = torch.zeros((G, n, n, self.cpad), dtype=dt, device=dev)

@@ -6,7 +6,7 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "libelfb200.so")
 
 INFO_FIELDS = 12
-FEAT_F32_NCHW, FEAT_F16_NHWC, FEAT_BF16_NHWC = 0, 1, 2  # ELFB200_FEAT_* (include/elfb200.h)
+FEAT_F32_NCHW, FEAT_F16_NHWC, FEAT_BF16_NHWC, FEAT_DF_F32_NCHW = 0, 1, 2, 3  # ELFB200_FEAT_* (include/elfb200.h)
 
 
 class ElfB200Error(RuntimeError):

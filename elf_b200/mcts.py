@@ -13,12 +13,16 @@ import numpy as np
 from . import lib as _l
 from .refstream import RefStreamSearch
 
+# planes of each leaf-batch format: the 18 AGZ planes, or the 25 DarkForest planes ("df")
+_PLANES = {"f32": 18, "f16": 18, "bf16": 18, "df": 25}
+
 
 class MctsBatch(RefStreamSearch):
     """``feature_format``: "f32" = the GoFeature contract, ``batch["s"]`` float32 ``[n,18,N,N]``
     (default); "f16" / "bf16" = the fast mode for a half-precision channels-last network: the leaf
     batch is written as ``batch["s_nhwc"]`` ``[n,N,N,cpad]`` (planes in channels 0..17, zeros above),
-    which ``elf_b200.model.FusedActor`` consumes without a cast/permute pass.
+    which ``elf_b200.model.FusedActor`` consumes without a cast/permute pass; "df" = the DarkForest planes
+    of ``GameOptions::use_df_feature``, ``batch["s"]`` float32 ``[n,25,N,N]`` (``BoardFeature::extract``).
     ``std_sort_ties=1`` (a search option like the others, ``include/elfb200_mcts.h``): moves whose network
     probabilities are bit-equal are stored in the order ``std::sort`` leaves them in inside the reference's
     ``pi2response`` instead of by ascending move -- needed to replay the reference's games exactly with a
@@ -32,8 +36,8 @@ class MctsBatch(RefStreamSearch):
 
         self.gb = go_batch
         self._lib = _l.load_library()
-        if feature_format not in ("f32", "f16", "bf16"):
-            raise ValueError("feature_format must be f32, f16 or bf16")
+        if feature_format not in _PLANES:
+            raise ValueError("feature_format must be f32, f16, bf16 or df")
         self.feature_format, self.cpad, self.strict_root = feature_format, int(cpad), bool(strict_root)
         self._mismatches = 0
         o = _l.MctsOptions()
@@ -61,21 +65,22 @@ class MctsBatch(RefStreamSearch):
     def set_feature_format(self, feature_format, cpad=None):
         """switch the leaf-batch format between moves/waves (re-allocates the feature tensor)"""
         torch = self._torch
-        if feature_format not in ("f32", "f16", "bf16"):
-            raise ValueError("feature_format must be f32, f16 or bf16")
+        if feature_format not in _PLANES:
+            raise ValueError("feature_format must be f32, f16, bf16 or df")
         self.gb.synchronize()
         self.feature_format = feature_format
         self.cpad = self.cpad if cpad is None else int(cpad)
         n = self.gb.board_size
         self.feat = None
-        if feature_format == "f32":
-            self._fmt = _l.FEAT_F32_NCHW
-            self.feat = torch.zeros((self.max_leaves, 18, n, n), dtype=torch.float32, device=self.device)
+        if feature_format in ("f32", "df"):
+            self._fmt = _l.FEAT_F32_NCHW if feature_format == "f32" else _l.FEAT_DF_F32_NCHW
+            self.feat = torch.zeros((self.max_leaves, _PLANES[feature_format], n, n), dtype=torch.float32,
+                                    device=self.device)
         else:
             self._fmt = _l.FEAT_F16_NHWC if feature_format == "f16" else _l.FEAT_BF16_NHWC
             dt = torch.float16 if feature_format == "f16" else torch.bfloat16
             self.feat = torch.zeros((self.max_leaves, n, n, self.cpad), dtype=dt, device=self.device)
-        self.feat_key = "s" if feature_format == "f32" else "s_nhwc"
+        self.feat_key = "s_nhwc" if feature_format in ("f16", "bf16") else "s"
 
     def close(self):
         if getattr(self, "_m", None):
@@ -111,7 +116,8 @@ class MctsBatch(RefStreamSearch):
 
     def select(self, wait=True):
         """one wave of descents; returns the CUDA feature tensor view of the leaves that need the
-        network (``[n,18,N,N]`` float32, or ``[n,N,N,cpad]`` in the 16-bit formats; n may be 0).
+        network (``[n,18,N,N]`` float32, ``[n,25,N,N]`` with "df", or ``[n,N,N,cpad]`` in the 16-bit
+        formats; n may be 0).
         ``wait=False``: nothing is read back and the host does not wait -- the view covers all
         ``max_leaves`` rows (rows past the device-side count are stale, their replies are ignored);
         ``leaf_count()`` fetches the count later."""

@@ -166,8 +166,13 @@ class OnlineGame:
         mcts_fields = {f[0] for f in _l.MctsOptions._fields_}
         mo = {k: kw.pop(k) for k in list(kw) if k in mcts_fields}
         mo.setdefault("komi", komi)
+        # use_df_feature (GameOptions::use_df_feature): the search's leaves and the human_actor position are
+        # the 25 DarkForest planes
+        df = bool(kw.pop("use_df_feature", False))
         gb = GoBatch(1, board_size=board_size, device=device)
-        return cls(gb, MctsBatch(gb, **mo), komi=komi, **kw)
+        game = cls(gb, MctsBatch(gb, feature_format="df" if df else "f32", **mo), komi=komi, **kw)
+        game.use_df_feature = df
+        return game
 
     # -- observers (GoGameSelfPlay::showBoard/getNextPlayer/getLastMove/getScore/getLastScore,
     #    common/game_selfplay.h:41-56) ---------------------------------------------------------

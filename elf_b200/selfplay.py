@@ -30,9 +30,21 @@ class SelfPlay:
                  resign_thres=0.05, never_resign_ratio=0.1, move_cutoff=-1, komi=7.5, seed=0,
                  record_games=False, actor_white=None, board=None, search=None, search_white=None,
                  white_mcts_opts=None, black_use_policy_network_only=False, white_use_policy_network_only=False,
-                 policy_distri_training_for_all=False, num_games_per_thread=-1, rng="numpy", **mcts_opts):
+                 policy_distri_training_for_all=False, num_games_per_thread=-1, rng="numpy", use_df_feature=False,
+                 **mcts_opts):
         # board / search / search_white: pre-built GoBatch / MctsBatch objects (or duck-typed stand-ins:
         # the CPU tests of the host logic inject oracle-backed ones); by default they are created here
+        # use_df_feature (GameOptions::use_df_feature): both AIs search on the 25 DarkForest planes, "s" float32
+        # [n,25,N,N] (a policy-only colour evaluates its root through the same leaf batch)
+        self.use_df_feature = bool(use_df_feature)
+        if self.use_df_feature:
+            for o in (mcts_opts, white_mcts_opts or {}):
+                if o.get("feature_format", "df") not in ("f32", "df"):
+                    raise ValueError("use_df_feature writes float32 DarkForest planes: feature_format "
+                                     f"{o['feature_format']!r} is not available with it")
+            mcts_opts["feature_format"] = "df"
+            if white_mcts_opts and "feature_format" in white_mcts_opts:
+                white_mcts_opts = {**white_mcts_opts, "feature_format": "df"}
         self.gb = board if board is not None else GoBatch(num_games, board_size=board_size, device=device)
         mcts_opts.setdefault("komi", komi)
         self._mcts_opts = dict(mcts_opts)

@@ -130,8 +130,14 @@ int elfb200_features_df_dev(elfb200_ctx* ctx, const int32_t* d4_dev, float* out_
 #define ELFB200_FEAT_F32_NCHW 0
 #define ELFB200_FEAT_F16_NHWC 1
 #define ELFB200_FEAT_BF16_NHWC 2
+/* ELFB200_FEAT_DF_F32_NCHW is the contract's other plane set: "s" as the 25 DarkForest planes of
+ * BoardFeature::extract (GameOptions::use_df_feature), float32 [n][25][N][N]; cpad is ignored.  The
+ * board batch (elfb200_features_dev_ex, the planes of elfb200_features_df_dev) and the search's leaf
+ * batch (elfb200_mcts_select_ex / elfb200_mcts_leaf_features) accept it. */
+#define ELFB200_FEAT_DF_F32_NCHW 3
 /* elfb200_features_dev with an explicit format.  out_dev: 16-byte aligned (float32: 8-byte aligned
- * is accepted, e.g. an odd row of a larger tensor, at the price of narrower stores). */
+ * is accepted, e.g. an odd row of a larger tensor, at the price of narrower stores; DarkForest float32:
+ * 4-byte aligned). */
 int elfb200_features_dev_ex(elfb200_ctx* ctx, const int32_t* d4_dev, void* out_dev, int format, int cpad);
 /* How the 16-bit NHWC planes are written: 0 = direct coalesced 16-byte vector stores (default; measured
  * 0.74 of the HBM copy peak), 1 = the position staged in shared memory and stored by one bulk (TMA,

@@ -86,7 +86,9 @@ int elfb200_mcts_begin_move(elfb200_mcts* m, const uint8_t* active_host);
 int elfb200_mcts_select(elfb200_mcts* m, float* feat_dev, int32_t* n_leaves);
 /* elfb200_mcts_select with an explicit feature format (ELFB200_FEAT_*, elfb200.h): the 16-bit
  * channels-last formats let a half-precision network read the leaf batch without a cast/permute
- * pass.  feat_dev: 16-byte aligned, capacity elfb200_mcts_max_leaves positions.
+ * pass; ELFB200_FEAT_DF_F32_NCHW writes the 25 DarkForest planes (GameOptions::use_df_feature) of every
+ * leaf instead of the 18 AGZ planes.  feat_dev: 16-byte aligned, capacity elfb200_mcts_max_leaves
+ * positions (DarkForest: max_leaves * 25*N*N floats).
  * n_leaves == NULL selects the ASYNCHRONOUS mode: nothing is copied back and the host does not
  * wait; the feature and expansion kernels run on a grid for all G*B slots and stop at the
  * device-side count, so the caller evaluates all elfb200_mcts_max_leaves rows (rows past the count

@@ -29,6 +29,8 @@ def main():
     ap.add_argument("--preload-sgf", default=None)
     ap.add_argument("--preload-sgf-move-to", type=int, default=-1)
     ap.add_argument("--device", type=int, default=0)
+    ap.add_argument("--use-df-feature", action="store_true",
+                    help="a DarkForest-plane network (GameOptions::use_df_feature): 25 input planes")
     args = ap.parse_args()
 
     import torch
@@ -38,7 +40,8 @@ def main():
     from elf_b200.online import OnlineGame
 
     torch.cuda.set_device(args.device)
-    net = PolicyValueNet(args.board, num_block=args.blocks, dim=args.dim).to(f"cuda:{args.device}")
+    net = PolicyValueNet(args.board, num_planes=25 if args.use_df_feature else 18, num_block=args.blocks,
+                         dim=args.dim).to(f"cuda:{args.device}")
     if args.load:
         sd = torch.load(args.load, map_location=f"cuda:{args.device}")
         missing, unexpected = load_reference_state_dict(net, sd)
@@ -50,7 +53,7 @@ def main():
         board_size=args.board, device=args.device, komi=args.komi, resign_thres=args.resign_thres,
         preload_sgf=args.preload_sgf, preload_sgf_move_to=args.preload_sgf_move_to, num_rollouts=args.rollouts,
         num_rollouts_per_batch=args.per_batch, c_puct=args.puct, virtual_loss=args.virtual_loss, persistent_tree=1,
-        rotation_flip=1)
+        rotation_flip=1, use_df_feature=args.use_df_feature)
     GtpConsole(game, actor).run()
 
 

@@ -39,6 +39,8 @@ def main():
     ap.add_argument("--moves", type=int, default=10, help="number of move-steps when --finish is 0")
     ap.add_argument("--records-out", default=None)
     ap.add_argument("--seed", type=int, default=0)
+    ap.add_argument("--use-df-feature", action="store_true",
+                    help="a DarkForest-plane network (GameOptions::use_df_feature): 25 input planes, float32 leaf batches")
     args = ap.parse_args()
 
     import torch
@@ -56,15 +58,18 @@ def main():
         os.environ.setdefault("MASTER_ADDR", "127.0.0.1")
         dist.init_process_group("nccl", device_id=torch.device("cuda", local))
     torch.manual_seed(args.seed)
-    net = PolicyValueNet(args.board, num_block=args.blocks, dim=args.dim).to(f"cuda:{local}")
+    planes = 25 if args.use_df_feature else 18
+    net = PolicyValueNet(args.board, num_planes=planes, num_block=args.blocks, dim=args.dim).to(f"cuda:{local}")
     if args.load and rank == 0:
         sd = torch.load(args.load, map_location=f"cuda:{local}")
         missing, unexpected = load_reference_state_dict(net, sd)
         print(f"[selfplay] loaded {args.load}: {len(missing)} missing / {len(unexpected)} unexpected keys", file=sys.stderr)
     broadcast_weights(net)
     # frozen-network inference engine: BatchNorm folded, fused cuDNN epilogues, a full NN batch as a CUDA graph;
-    # the search hands it the leaf batch as fp16 channels-last (no cast/permute pass)
-    actor = FusedActor(net.eval(), batchsize=args.nn_batch, dtype=torch.float16, cuda_graph=True)
+    # the search hands it the leaf batch as fp16 channels-last (no cast/permute pass); the DarkForest planes come
+    # as float32 "s" and are converted in one pass into 32 padded channels
+    actor = FusedActor(net.eval(), batchsize=args.nn_batch, dtype=torch.float16, cuda_graph=True,
+                       cpad=32 if args.use_df_feature else 24)
     sp = elf_b200.selfplay.SelfPlay(
         actor, num_games=args.games, board_size=args.board, device=local,
         policy_distri_cutoff=args.policy_distri_cutoff, resign_thres=args.resign_thres,
@@ -72,7 +77,7 @@ def main():
         record_games=args.records_out is not None, num_rollouts=args.rollouts,
         num_rollouts_per_batch=args.per_batch, c_puct=args.puct, virtual_loss=args.virtual_loss,
         persistent_tree=1, root_epsilon=args.root_epsilon, root_alpha=args.root_alpha, rotation_flip=1,
-        feature_format="f16")
+        **({"use_df_feature": True} if args.use_df_feature else {"feature_format": "f16"}))
     t0 = time.perf_counter()
     steps = 0
     while (sp.games_finished < args.finish) if args.finish > 0 else (steps < args.moves):
