@@ -110,7 +110,8 @@ class GoBatch:
         i as it is.  ``index``: G entries, a list / numpy array (synchronous), or an int32 CUDA tensor on
         this batch's device (asynchronous: ordered after the caller's current stream and before its next
         work, with events only, so it can be captured in a CUDA graph).  A search handle on this batch keeps
-        its trees: reset the copied games' trees before their next search."""
+        its trees: copy them with the same index (``MctsBatch.gather``) or reset the copied games' trees
+        before their next search."""
         if getattr(index, "is_cuda", False):
             return self._gather_dev(src, index)
         a = np.asarray(index)

@@ -451,6 +451,19 @@ int elfb200_fail(int code, const char* fmt, ...);  // records the message for el
     }                                  \
   } while (0)
 
+// `waiter`'s later work runs after the work already on `first` (event `ev`); used by the copies between two
+// contexts or two search handles.  The SIMT emulator build runs all work in issue order, so there it has
+// nothing to order.
+static inline int stream_after(cudaStream_t waiter, cudaStream_t first, cudaEvent_t ev) {
+#if defined(ELFB200_SIMT_EMU)
+  (void)waiter, (void)first, (void)ev;
+#else
+  CK(cudaEventRecord(ev, first));
+  CK(cudaStreamWaitEvent(waiter, ev, 0));
+#endif
+  return ELFB200_OK;
+}
+
 struct elfb200_ctx {
   int N = 0, G = 0, device = 0;
   cudaStream_t stream = nullptr;
@@ -485,7 +498,8 @@ struct elfb200_ctx {
   size_t map_ok_off = 0, map_flag_off = 0;  // byte offsets of the accept flags / completion flag in the mapped window
   uint32_t step_seq = 0;        // sequence number the last CTA writes into the mapped completion flag
   int64_t launches = 0;
-  // fork / join of elfb200_gather_games_dev with this context as the destination (cudaEventDisableTiming)
+  // fork / join of elfb200_gather_games_dev and elfb200_mcts_gather_dev with this context as the destination
+  // (cudaEventDisableTiming)
   cudaEvent_t ev_gather[2] = {nullptr, nullptr};
   // move lists of elfb200_replay (grown on demand)
   int16_t* d_replay = nullptr;

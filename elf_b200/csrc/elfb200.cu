@@ -1455,18 +1455,6 @@ static int check_gather(const elfb200_ctx* dst, const elfb200_ctx* src, const in
   return ELFB200_OK;
 }
 
-// `waiter`'s later work runs after the work already on `first` (event `ev`).  The SIMT emulator build runs all
-// work in issue order, so there it has nothing to order.
-static int stream_after(cudaStream_t waiter, cudaStream_t first, cudaEvent_t ev) {
-#if defined(ELFB200_SIMT_EMU)
-  (void)waiter, (void)first, (void)ev;
-#else
-  CK(cudaEventRecord(ev, first));
-  CK(cudaStreamWaitEvent(waiter, ev, 0));
-#endif
-  return ELFB200_OK;
-}
-
 // k_gather on dst's stream, after the work already on src's stream (fork); src's later work waits for the
 // copy (join), so it cannot change a game while the game is read
 static int gather_launch(elfb200_ctx* dst, const elfb200_ctx* src, const int32_t* index_dev) {

@@ -25,7 +25,8 @@
 // Kernels: k_begin (root set-up), k_select (PUCT descent + child state creation + terminal
 // evaluation + leaf claim), k_leaf_features (18-plane stack per claimed leaf, history gathered
 // along the parent chain; k_leaf_features_df: the 25 DarkForest planes instead), k_expand (mask/sort/renormalise the net's policy into edges),
-// k_backup, k_results, k_advance (tree reuse: keep the chosen child's subtree, free the rest).
+// k_backup, k_results, k_advance (tree reuse: keep the chosen child's subtree, free the rest),
+// k_gather_trees (copy trees from another handle's pool, node for node).
 #include <cfloat>
 
 #include "common.cuh"
@@ -1435,6 +1436,109 @@ __global__ void k_tree_reset(int G, TreeDev tr, const uint8_t* __restrict__ mask
   }
 }
 
+// ---------------------------------------------------------------------------------------
+// Copy search trees from another handle's pool (elfb200_mcts_gather): destination game i gets an exact replica
+// of source game index[i]'s tree for index[i] in [0, G_src); any other value leaves game i as it is.  Local ids
+// are kept, so nothing is renumbered: the root, the free stack free_list[0 .. free_n) verbatim (later
+// allocations pop the same ids), and for every in-use node (status != NS_FREE) its pos / sa rows, hash, meta
+// and header; for every visited node the edges [0, n_edges) of estat and elink.  Free slots and edges past
+// n_edges are not copied: no kernel reads them (DESIGN §3 "Copying games").  A slot the source has free only
+// gets status NS_FREE, as k_advance / free_subtree leave freed slots: every slot on the free stack and no
+// other is NS_FREE, which a later copy of this tree and elfb200_mcts_tree_usage rely on.
+// One CTA per destination game (1.4x faster than one warp per game on an H100, DESIGN §5.2); warp w takes the
+// 32-node chunks w, w + 8, ...: each lane reads one node's header and copies that node's small records, the
+// warp copies the chunk's position rows (contiguous) and then the edges of each visited node, up to four
+// 16-byte records per lane in flight.
+constexpr int TREE_GATHER_THREADS = 256;
+
+template <class T>
+__device__ __forceinline__ void copy_run(T* __restrict__ d, const T* __restrict__ s, int n, int lane) {
+  int i = lane;
+  for (; i + 96 < n; i += 128) {
+    const T a = __ldg(s + i), b = __ldg(s + i + 32), c = __ldg(s + i + 64), e = __ldg(s + i + 96);
+    d[i] = a;
+    d[i + 32] = b;
+    d[i + 64] = c;
+    d[i + 96] = e;
+  }
+  for (; i < n; i += 32) d[i] = __ldg(s + i);
+}
+
+template <int N>
+__global__ void __launch_bounds__(TREE_GATHER_THREADS)
+    k_gather_trees(TreeDev dst, TreeDev src, int G_dst, int G_src, const int32_t* __restrict__ index) {
+  const int gd = blockIdx.x;
+  if (gd >= G_dst) return;
+  const int gs = __ldg(index + gd);
+  if (gs < 0 || gs >= G_src) return;
+  const int C = dst.C, E = dst.E;
+  const size_t nd = (size_t)gd * C, ns = (size_t)gs * C;
+  const int lane = threadIdx.x & 31, nwarps = blockDim.x >> 5;
+  const int nfree = min(max(__ldg(src.free_n + gs), 0), C);
+  for (int i = threadIdx.x; i < nfree; i += blockDim.x) dst.free_list[nd + i] = __ldg(src.free_list + ns + i);
+  if (threadIdx.x == 0) {
+    dst.free_n[gd] = nfree;
+    dst.root[gd] = __ldg(src.root + gs);
+  }
+  for (int c0 = (threadIdx.x >> 5) * 32; c0 < C; c0 += nwarps * 32) {
+    const int v = c0 + lane;
+    NodeHdr h = {};
+    if (v < C) h = load_hdr(&src.hdr[ns + v]);
+    const bool used = v < C && h.status != NS_FREE;
+    const int ne = used && h.status == NS_VISITED ? min((int)h.n_edges, E) : 0;
+    const uint32_t used_mask = __ballot_sync(FULL, used), vis_mask = __ballot_sync(FULL, ne > 0);
+    if (used) {
+      store_hdr(&dst.hdr[nd + v], h);
+      dst.hash[nd + v] = __ldg(src.hash + ns + v);
+      store_meta(&dst.meta[nd + v], load_meta(&src.meta[ns + v]));
+    } else if (v < C) {
+      dst.hdr[nd + v].status = NS_FREE;  // the pool's invariant: exactly the slots on the free stack are NS_FREE
+    }
+    // position and group-status rows of the chunk's in-use nodes: 32 N contiguous words each
+    const int nrow = min(32, C - c0) * N;
+    for (int k = lane; k < nrow; k += 32) {
+      if ((used_mask >> (k / N)) & 1u) {
+        dst.pos[(nd + c0) * N + k] = __ldg(src.pos + (ns + c0) * N + k);
+        dst.sa[(nd + c0) * N + k] = __ldg(src.sa + (ns + c0) * N + k);
+      }
+    }
+    // edges of the visited nodes: estat in 16-byte records, elink in pairs (its rows are 8-byte aligned)
+    for (uint32_t m = vis_mask; m; m &= m - 1) {
+      const int l = __ffs(m) - 1;
+      const int cnt = __shfl_sync(FULL, ne, l);
+      const size_t od = (nd + c0 + l) * E, os = (ns + c0 + l) * E;
+      copy_run(dst.estat + od, src.estat + os, cnt, lane);
+      copy_run(reinterpret_cast<uint2*>(dst.elink + od), reinterpret_cast<const uint2*>(src.elink + os), cnt >> 1, lane);
+      if ((cnt & 1) && lane == 0) dst.elink[od + cnt - 1] = __ldg(src.elink + os + cnt - 1);
+    }
+  }
+}
+
+// In-use nodes and stored edges of the visited nodes of every game's tree (elfb200_mcts_tree_usage): what
+// k_gather_trees moves for the game.  One warp per game.
+__global__ void __launch_bounds__(BLOCK) k_tree_usage(int G, TreeDev tr, int32_t* __restrict__ nodes,
+                                                      int32_t* __restrict__ edges) {
+  const int lane = threadIdx.x & 31;
+  const int g = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+  if (g >= G) return;
+  const size_t nb = (size_t)g * tr.C;
+  int nu = 0, ne = 0;
+  for (int i = lane; i < tr.C; i += 32) {
+    const NodeHdr h = load_hdr(&tr.hdr[nb + i]);
+    nu += h.status != NS_FREE;
+    ne += h.status == NS_VISITED ? (int)h.n_edges : 0;
+  }
+#pragma unroll
+  for (int d = 16; d > 0; d >>= 1) {
+    nu += __shfl_xor_sync(FULL, nu, d);
+    ne += __shfl_xor_sync(FULL, ne, d);
+  }
+  if (lane == 0) {
+    nodes[g] = nu;
+    edges[g] = ne;
+  }
+}
+
 __global__ void k_leaf_info(TreeDev tr, uint64_t* __restrict__ hash, int32_t* __restrict__ game,
                             int32_t* __restrict__ ply, int32_t* __restrict__ d4) {
   const int s = blockIdx.x * blockDim.x + threadIdx.x;
@@ -1487,6 +1591,7 @@ struct elfb200_mcts {
   cudaEvent_t ev[7] = {};  // sel0 sel1 feat0 feat1 exp0 exp1 bak1
   bool pending_sel = false, pending_feat = false, pending_eb = false;
   bool used_async = false;  // a wave ran without the host reading its leaf count
+  bool wave_open = false;   // select issued, expand_backup not yet: nodes are claimed and virtual loss is applied
   double acc_ms[4] = {0, 0, 0, 0};  // select, features, expand, backup
   int64_t acc_waves = 0;
 };
@@ -1741,6 +1846,7 @@ int elfb200_mcts_select_ex(elfb200_mcts* m, void* feat_dev, int format, int cpad
   CK(cudaGetLastError());
   CK(cudaEventRecord(m->ev[1], c->stream));
   m->pending_sel = true;
+  m->wave_open = true;
   int n = -1;  // unknown to the host: the feature / expand grids cover all G*B slots and the kernels
                // stop at the device-side count
   if (n_leaves) {
@@ -1841,6 +1947,7 @@ int elfb200_mcts_expand_backup(elfb200_mcts* m, const float* pi_dev, const float
   CK(cudaGetLastError());
   CK(cudaEventRecord(m->ev[6], c->stream));
   m->pending_eb = true;
+  m->wave_open = false;
   return ELFB200_OK;
 }
 
@@ -2033,6 +2140,71 @@ int elfb200_mcts_timings(elfb200_mcts* m, double* ms_host4, int64_t* waves, int 
     for (int i = 0; i < 4; ++i) m->acc_ms[i] = 0;
     m->acc_waves = 0;
   }
+  return ELFB200_OK;
+}
+
+static int check_tree_gather(const elfb200_mcts* dst, const elfb200_mcts* src, const int32_t* index) {
+  if (!dst || !src || !index) return elfb200_fail(ELFB200_ERR_ARG, "dst/src/index is NULL");
+  if (dst == src)
+    return elfb200_fail(ELFB200_ERR_ARG, "dst and src are the same search handle (an in-place permutation would race)");
+  const elfb200_ctx *cd = dst->ctx, *cs = src->ctx;
+  if (cd->N != cs->N) return elfb200_fail(ELFB200_ERR_ARG, "board sizes differ (dst %d, src %d)", cd->N, cs->N);
+  if (cd->device != cs->device) return elfb200_fail(ELFB200_ERR_ARG, "devices differ (dst %d, src %d)", cd->device, cs->device);
+  if (dst->tr.C != src->tr.C)
+    return elfb200_fail(ELFB200_ERR_ARG, "nodes_per_game differs (dst %d, src %d)", dst->tr.C, src->tr.C);
+  if (dst->wave_open || src->wave_open)
+    return elfb200_fail(ELFB200_ERR_ARG, "the %s handle has a wave open (select without expand_backup)",
+                        dst->wave_open ? "dst" : "src");
+  return ELFB200_OK;
+}
+
+// k_gather_trees on dst's stream, after the work already on src's stream (fork); src's later work waits for the
+// copy (join), so it cannot change a tree while the tree is read.  Two handles on one context share the stream.
+// The fork / join events are the destination context's, the two of elfb200_gather_games_dev: each record is
+// waited on before the next call records it again, so the board copy and the tree copy can share them, and a
+// search handle allocates nothing for copies it never makes.
+static int tree_gather_launch(elfb200_mcts* dst, const elfb200_mcts* src, const int32_t* index_dev) {
+  elfb200_ctx *cd = dst->ctx, *cs = src->ctx;
+  int rc = stream_after(cd->stream, cs->stream, cd->ev_gather[0]);
+  if (rc) return rc;
+  DISPATCH_N(cd,
+             (k_gather_trees<19><<<cd->G, TREE_GATHER_THREADS, 0, cd->stream>>>(dst->tr, src->tr, cd->G, cs->G, index_dev)),
+             (k_gather_trees<9><<<cd->G, TREE_GATHER_THREADS, 0, cd->stream>>>(dst->tr, src->tr, cd->G, cs->G, index_dev)));
+  cd->launches++;
+  CK(cudaGetLastError());
+  return stream_after(cs->stream, cd->stream, cd->ev_gather[1]);
+}
+
+int elfb200_mcts_gather_dev(elfb200_mcts* dst, const elfb200_mcts* src, const int32_t* index_dev) {
+  int rc = check_tree_gather(dst, src, index_dev);
+  if (rc) return rc;
+  CK(cudaSetDevice(dst->ctx->device));
+  return tree_gather_launch(dst, src, index_dev);
+}
+
+int elfb200_mcts_gather(elfb200_mcts* dst, const elfb200_mcts* src, const int32_t* index_host) {
+  int rc = check_tree_gather(dst, src, index_host);
+  if (rc) return rc;
+  elfb200_ctx* c = dst->ctx;
+  CK(cudaSetDevice(c->device));
+  memcpy(c->h_pin, index_host, (size_t)c->G * 4);
+  CK(cudaMemcpyAsync(dst->d_actions, c->h_pin, (size_t)c->G * 4, cudaMemcpyHostToDevice, c->stream));
+  rc = tree_gather_launch(dst, src, dst->d_actions);
+  if (rc) return rc;
+  CK(cudaStreamSynchronize(c->stream));
+  return ELFB200_OK;
+}
+
+int elfb200_mcts_tree_usage(elfb200_mcts* m, int32_t* nodes_host, int32_t* edges_host) {
+  if (!m || !nodes_host || !edges_host) return elfb200_fail(ELFB200_ERR_ARG, "NULL argument");
+  elfb200_ctx* c = m->ctx;
+  CK(cudaSetDevice(c->device));
+  k_tree_usage<<<warp_grid(c->G), BLOCK, 0, c->stream>>>(c->G, m->tr, m->d_best, m->d_total);
+  c->launches++;
+  CK(cudaGetLastError());
+  CK(cudaMemcpyAsync(nodes_host, m->d_best, (size_t)c->G * 4, cudaMemcpyDeviceToHost, c->stream));
+  CK(cudaMemcpyAsync(edges_host, m->d_total, (size_t)c->G * 4, cudaMemcpyDeviceToHost, c->stream));
+  CK(cudaStreamSynchronize(c->stream));
   return ELFB200_OK;
 }
 

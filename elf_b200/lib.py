@@ -104,6 +104,9 @@ SIGNATURES = {
     "elfb200_mcts_eval_count": (ctypes.c_int64, [vp]),
     "elfb200_mcts_stats": (ctypes.c_int, [vp, vp]),
     "elfb200_mcts_timings": (ctypes.c_int, [vp, vp, vp, ctypes.c_int]),
+    "elfb200_mcts_gather": (ctypes.c_int, [vp, vp, vp]),
+    "elfb200_mcts_gather_dev": (ctypes.c_int, [vp, vp, vp]),
+    "elfb200_mcts_tree_usage": (ctypes.c_int, [vp, vp, vp]),
 }
 
 

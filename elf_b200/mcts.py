@@ -191,6 +191,59 @@ class MctsBatch(RefStreamSearch):
         a = np.ascontiguousarray(actions, dtype=np.int32)
         _l.check(self._lib, self._lib.elfb200_mcts_advance(self._m, a.ctypes.data))
 
+    # -- copying trees between handles -----------------------------------------------------------
+    def gather(self, src, index):
+        """copy search trees from the handle ``src`` (same board size and ``nodes_per_game``, not this handle;
+        it may search the same GoBatch): game i's tree becomes an exact replica of src's game ``index[i]`` for
+        ``index[i]`` in [0, src's number of games); any other value leaves game i's tree as it is.  Continued
+        search on a copy is bitwise the search its source would run.  The random state of each game (D4 codes,
+        root noise) stays with this handle.  ``index`` as in ``GoBatch.gather``: a list / numpy array
+        (synchronous) or a contiguous int32 CUDA tensor on this handle's device (asynchronous: ordered after the
+        caller's current stream and before its next work, with events only, so it can be captured in a CUDA
+        graph).  Not while either handle has a wave open (``select`` without ``expand_backup``).
+
+        Copy the boards with the same index first (``GoBatch.gather`` / ``GoEnv.load``): the next
+        ``begin_move`` checks every root against its board, so a tree whose board was not copied raises with
+        ``strict_root`` or is counted in ``errors()[0]`` and rebuilt from the board."""
+        if getattr(index, "is_cuda", False):
+            return self._gather_dev(src, index)
+        G = self.gb.num_games
+        a = np.asarray(index)
+        if a.dtype != np.int32:  # out-of-range values stay out of range (untouched games) in int32
+            a = np.clip(a, -1, src.gb.num_games)
+        a = np.ascontiguousarray(a, dtype=np.int32)
+        if a.shape != (G,):
+            raise ValueError(f"index must have shape ({G},), got {a.shape}")
+        _l.check(self._lib, self._lib.elfb200_mcts_gather(self._m, src._m, a.ctypes.data))
+
+    def _gather_dev(self, src, index):
+        torch = self._torch
+        G = self.gb.num_games
+        if index.dtype != torch.int32 or tuple(index.shape) != (G,) or not index.is_contiguous() \
+                or index.device != self.device:
+            raise ValueError(f"index must be a contiguous int32 tensor of shape ({G},) on {self.device}")
+        if getattr(self, "_gather_ev", None) is None:
+            self._gather_ev = [torch.cuda.Event() for _ in range(3)]
+        ev, s_dst, s_src = self._gather_ev, self._stream, src._stream
+        cur = torch.cuda.current_stream(self.device)
+        # both context streams join the caller's stream before the copy and rejoin it afterwards
+        ev[0].record(cur)
+        s_dst.wait_event(ev[0])
+        s_src.wait_event(ev[0])
+        _l.check(self._lib, self._lib.elfb200_mcts_gather_dev(self._m, src._m, index.data_ptr()))
+        ev[1].record(s_dst)
+        cur.wait_event(ev[1])
+        ev[2].record(s_src)
+        cur.wait_event(ev[2])
+
+    def tree_usage(self):
+        """(nodes, edges) int32 [G] each: in-use nodes and stored edges of the visited nodes of every game's
+        tree, the records ``gather`` copies for the game"""
+        G = self.gb.num_games
+        nodes, edges = np.zeros(G, np.int32), np.zeros(G, np.int32)
+        _l.check(self._lib, self._lib.elfb200_mcts_tree_usage(self._m, nodes.ctypes.data, edges.ctypes.data))
+        return nodes, edges
+
     def root_priors(self):
         """float32 [G, N*N+1]: prior of every root edge by action, -1 where there is no edge"""
         o = np.empty((self.gb.num_games, self.gb.num_actions), np.float32)

@@ -161,6 +161,24 @@ int elfb200_mcts_stats(elfb200_mcts* m, uint64_t* counters_host4);
  * leaf-feature, expand and backup kernels, and the number of waves they cover; reset != 0 clears. */
 int elfb200_mcts_timings(elfb200_mcts* m, double* ms_host4, int64_t* waves, int reset);
 
+/* Copy search trees from another handle, node for node: dst game i gets an exact replica of src game
+ * index[i]'s tree (root, free stack, every in-use node, the edges of every visited node) for index[i] in
+ * [0, G_src); any other value leaves game i's tree as it is.  The random state of each game (D4 codes, root
+ * noise), the counters and the per-wave buffers stay with dst.  Copy the boards with the same index first
+ * (elfb200_gather_games): the next begin_move checks each root against its board.
+ * Same board size and nodes_per_game; dst != src, but both may search the same board context (two AIs with
+ * a tree per colour).  ELFB200_ERR_ARG, with nothing enqueued, for NULL arguments, dst == src, different
+ * board sizes, devices or pool sizes, and when either handle has a wave open (select issued, expand_backup
+ * not yet).
+ * _gather: host index int32[G_dst], synchronous.  _gather_dev: device index int32[G_dst], asynchronous on
+ * dst's context stream, after the work already on src's stream; src's later work runs after the copy
+ * (the two timing-free events of dst's board context that elfb200_gather_games_dev uses), so it can be captured in a CUDA graph that holds both streams. */
+int elfb200_mcts_gather(elfb200_mcts* dst, const elfb200_mcts* src, const int32_t* index_host);
+int elfb200_mcts_gather_dev(elfb200_mcts* dst, const elfb200_mcts* src, const int32_t* index_dev);
+/* int32[G] each (host): in-use nodes, and stored edges of the visited nodes, of every game's tree -- what
+ * elfb200_mcts_gather copies for the game. */
+int elfb200_mcts_tree_usage(elfb200_mcts* m, int32_t* nodes_host, int32_t* edges_host);
+
 #ifdef __cplusplus
 }
 #endif
