@@ -335,10 +335,12 @@ class GoBatch:
         cur.wait_event(ev[1])
         return out
 
-    def final_status(self, counts=None, playouts=None, threshold=0.5):
+    def final_status(self, counts=None, playouts=None, threshold=0.5, pass_alive=False):
         """dead groups and getTrompTaylorScore of every stored position.  With ``counts`` (``ownership``'s
         result over ``playouts`` playouts) a group is dead when its stones' mean ownership margin for its own
-        colour, (own - opponent) / playouts, is below ``-threshold``; without counts no group is dead.  Returns
+        colour, (own - opponent) / playouts, is below ``-threshold``; without counts no group is dead.
+        ``pass_alive=True`` adds the exact rule of ``pass_alive``: pass-alive stones are never dead, and the
+        opponent's stones inside a pass-alive area always are (without counts that is the whole rule).  Returns
         ``(dead, territory, score)``: uint8 ``[G, N*N]`` 1 on dead stones, uint8 ``[G, N*N]`` 1 black / 2 white /
         3 dame with dead stones counted for the opponent, int32 ``[G]`` black minus white (no komi)."""
         n, G = self.board_size, self.num_games
@@ -353,7 +355,8 @@ class GoBatch:
         dead = np.empty((G, n * n), np.uint8)
         terr = np.empty((G, n * n), np.uint8)
         score = np.empty(G, np.int32)
-        _l.check(self._lib, self._lib.elfb200_final_status(
+        fn = self._lib.elfb200_final_status_pass_alive if pass_alive else self._lib.elfb200_final_status
+        _l.check(self._lib, fn(
             self._ctx, c.ctypes.data if c is not None else None, K, float(threshold), dead.ctypes.data,
             terr.ctypes.data, score.ctypes.data))
         return dead, terr, score
@@ -399,6 +402,50 @@ class GoBatch:
         s.wait_event(ev[0])
         _l.check(self._lib, self._lib.elfb200_tactics_dev(self._ctx, ladder.data_ptr() if ladder is not None else None,
                                                           sa.data_ptr() if sa is not None else None))
+        ev[1].record(s)
+        cur.wait_event(ev[1])
+        return out
+
+    # -- pass-alive chains and areas -------------------------------------------------------------
+    def pass_alive(self, out=None):
+        """Benson's unconditional life for both colours, by action x*N+y.  Returns ``(alive, area)``, uint8
+        ``[G, N*N]`` each: ``alive`` is 1 on every stone of a chain that cannot be captured even if its owner
+        passes forever (the stone's colour says whose); ``area`` is 1 / 2 on the points of black's / white's
+        pass-alive area (the enclosed regions vital to those chains; opponent stones there are dead with
+        certainty), 0 elsewhere.  Only the position is read, not the history, ko or side to move.  With
+        ``out=(alive, area)``, contiguous uint8 CUDA tensors of shape ``[G, N*N]`` on this batch's device (either
+        may be None, and its work is skipped), the values are written there asynchronously, ordered after the
+        caller's current stream and before its next work with events only (capturable in a CUDA graph); ``out``
+        is returned.  The stored games stay as they are."""
+        n, G = self.board_size, self.num_games
+        if out is not None:
+            return self._pass_alive_dev(out)
+        alive = np.empty((G, n * n), np.uint8)
+        area = np.empty((G, n * n), np.uint8)
+        _l.check(self._lib, self._lib.elfb200_pass_alive(self._ctx, alive.ctypes.data, area.ctypes.data))
+        return alive, area
+
+    def _pass_alive_dev(self, out):
+        import torch
+
+        dev = torch.device("cuda", self.device)
+        n = self.board_size
+        alive, area = out
+        for t in (alive, area):
+            if t is not None and (not isinstance(t, torch.Tensor) or t.dtype != torch.uint8
+                                  or tuple(t.shape) != (self.num_games, n * n) or not t.is_contiguous()
+                                  or t.device != dev):
+                raise ValueError(f"out must hold contiguous uint8 tensors of shape ({self.num_games}, {n * n}) "
+                                 f"on {dev}, or None")
+        if getattr(self, "_pa_ev", None) is None:
+            self._pa_ev = [torch.cuda.Event() for _ in range(2)]
+            self._pa_stream = torch.cuda.ExternalStream(self.stream, device=dev)
+        ev, s = self._pa_ev, self._pa_stream
+        cur = torch.cuda.current_stream(dev)
+        ev[0].record(cur)
+        s.wait_event(ev[0])
+        _l.check(self._lib, self._lib.elfb200_pass_alive_dev(self._ctx, alive.data_ptr() if alive is not None else None,
+                                                             area.data_ptr() if area is not None else None))
         ev[1].record(s)
         cur.wait_event(ev[1])
         return out

@@ -20,7 +20,9 @@ Beyond ``console_lib.py``, three GTP 2 commands start a handicap game: ``fixed_h
 per line (vertices ascending, groups by their lowest vertex).  Dead groups come from Monte-Carlo ownership
 (``OnlineGame.final_status``: 1024 random playouts from the position); ``seki`` is always empty, there is no
 seki detection.  It is offered when the board behind the game can play those playouts
-(``GoBatch.ownership``).
+(``GoBatch.ownership``).  With ``final_status_pass_alive = True`` (``scripts/gtp.py --pass-alive``) the
+playout rule is combined with Benson's exact one: pass-alive groups are never listed dead, and opponent stones
+inside a pass-alive area always are (``GoBatch.pass_alive``).
 
 The reference console talks to its game thread by returning special actions from the
 ``human_actor`` callback; here the same special actions go straight into ``OnlineGame.human``.
@@ -64,6 +66,7 @@ class GtpConsole:
         if getattr(game.board, "ownership", None) is None:  # a board that cannot play ownership playouts
             del self.commands["final_status_list"]
         self.final_status_playouts = 1024
+        self.final_status_pass_alive = False  # True: combine the playout rule with the pass-alive rule
 
     # -- helpers ---------------------------------------------------------------------------------
     def check_player(self, player):  # console_lib.py:313-325
@@ -178,7 +181,10 @@ class GtpConsole:
             return False, "syntax error"
         if status == "seki":  # no seki detection
             return True, ""
-        dead, alive = self.game.final_status(playouts=self.final_status_playouts)
+        if self.final_status_pass_alive:
+            dead, alive = self.game.final_status(playouts=self.final_status_playouts, pass_alive=True)
+        else:
+            dead, alive = self.game.final_status(playouts=self.final_status_playouts)
         groups = dead if status == "dead" else alive
         return True, "\n".join(" ".join(_o.action2vertex(a, self.board_size) for a in g) for g in groups)
 

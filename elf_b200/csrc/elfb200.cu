@@ -13,8 +13,10 @@
 //   k_playout2  k_playout in the two-rows-per-lane layout (board2.cuh), 19x19 only
 //   k_gather    copy games from another batch (GoState's copy constructor); no geometry, one kernel for both sizes
 //   k_ownership K random-policy playouts from every stored position, per-point area counts (Monte-Carlo ownership)
-//   k_final_status  dead groups from those counts, getTrompTaylorScore with them (territory map and score)
+//   k_final_status  dead groups from those counts, getTrompTaylorScore with them (territory map and score);
+//               k_final_status<N, true> adds the pass-alive rule (k_pass_alive's analysis)
 //   k_tactics   checkLadder and isSelfAtari for every point and both colours (ladder depth, self-atari size)
+//   k_pass_alive  Benson's pass-alive chains and areas of both colours (no reference counterpart)
 //
 // Each game rule lives in one device function that the kernels share: forward_ply is GoState::forward's move
 // (k_step, k_env_step, k_replay), random_ply one move of the random policy (k_playout, k_playout2, k_ownership),
@@ -845,6 +847,203 @@ __global__ void __launch_bounds__(PLAYOUT_WARPS * 32)
 }
 
 // ---------------------------------------------------------------------------------------
+// Pass-alive chains and areas (Benson 1976) of every stored position, both colours (elfb200_pass_alive; also the
+// exact part of k_final_status<N, true>).  For a colour c: chains are the maximal 4-connected sets of c stones,
+// regions the maximal 4-connected sets of points without a c stone.  A region is vital to a chain when every
+// empty point of the region is a liberty of the chain.  Starting from every chain in X and every region in R,
+// repeat until nothing changes: drop from X every chain with fewer than two regions of R vital to it, then drop
+// from R every region that borders a chain no longer in X.  Pass-alive stones: those of the chains left in X;
+// pass-alive area: every point of a region left in R that is vital to a chain left in X.  The position is all
+// that is read (no history, ko or side to move).  The reference has no counterpart (DESIGN §3).
+//
+// One warp per game, one row per lane (make_lane_single).  Per colour: chains are labelled one at a time by
+// seed-ballot link fills (ids in shared memory), then regions by plain fills within the non-c mask.  A region is
+// vital only to chains next to its first empty point (at most four ids kept per region), and to none unless
+// every one of its empty points touches a c stone.  Step 1 runs on per-chain counters, lane-parallel; step 2 is
+// one fill: the live region points next to removed chains' stones, grown within the live regions, are exactly
+// the regions to drop, and each dropped region (found by its seed point) takes one off its vital chains' counters.
+// Chains of one colour are pairwise non-adjacent, so one point of each is an independent set of the grid and
+// there are at most ceil(N*N / 2) of them; regions likewise.
+// delta4 (also the ladder reader's) (board.h:220): (x-1, y), (x, y-1), (x+1, y), (x, y+1)
+__device__ __forceinline__ int d4x(int d) { return d == 0 ? -1 : d == 2 ? 1 : 0; }
+__device__ __forceinline__ int d4y(int d) { return d == 1 ? -1 : d == 3 ? 1 : 0; }
+
+// Point (x, y) of the row words v, false off the board.  Warp-uniform: every lane gets row y by a shuffle.
+template <int N>
+__device__ __forceinline__ bool bit_at(uint32_t v, int x, int y) {
+  const bool on = x >= 0 && x < N && y >= 0 && y < N;
+  const uint32_t r = __shfl_sync(FULL, v, on ? y : 0);
+  return on && ((r >> x) & 1u);
+}
+
+constexpr int PA_WARPS = 4;  // games per CTA of k_pass_alive
+template <int N>
+struct PaScratch {
+  static constexpr int MAXK = (N * N + 1) / 2;  // chains or regions of one colour
+  uint32_t rows[2][32];   // row words passed between lanes
+  int32_t cnt[MAXK];      // per chain: regions of R vital to it
+  int16_t seed[MAXK];     // per region: its first point p = y*N + x
+  uint8_t vit[MAXK][4];   // per region: the chains it is vital to, 0xFF where none
+  uint8_t cid[N * N];     // per own stone p: its chain
+  uint8_t gone[MAXK];     // per chain: dropped from X
+};
+
+// Own stones of the chains not dropped: the bits of `m` (own stones of this row) whose chain is (not) gone.
+template <int N>
+__device__ __forceinline__ uint32_t pa_chain_rows(uint32_t m, const PaScratch<N>& s, const Lane& L, bool gone) {
+  uint32_t r = 0;
+  for (; m; m &= m - 1) {
+    const int x = __ffs(m) - 1;
+    if ((s.gone[s.cid[L.row * N + x]] != 0) == gone) r |= 1u << x;
+  }
+  return r;
+}
+
+// Benson's analysis for the colour whose stones are `own`; `opp` the other colour's.
+template <int N>
+__device__ __forceinline__ void pass_alive_colour(uint32_t own, uint32_t opp, PaScratch<N>& s, const Lane& L,
+                                                  uint32_t& alive, uint32_t& area) {
+  const uint32_t non = ~own & L.rm, e = non & ~opp;
+  __syncwarp();  // the scratch may still be read by the previous call
+  // chains
+  const Links lk = make_links<N>(own, 0u, L);
+  int nc = 0;
+  for (uint32_t left = own;; ++nc) {
+    const unsigned lanes = __ballot_sync(FULL, left != 0u);
+    if (!lanes) break;
+    const int src = __ffs(lanes) - 1;
+    uint32_t grp = L.lane == src ? (left & (0u - left)) : 0u;
+    while (true) {
+      const uint32_t n2 = grow_link(grow_link(grp, lk), lk);
+      const bool ch = n2 != grp;
+      grp = n2;
+      if (!__any_sync(FULL, ch)) break;
+    }
+    for (uint32_t m = grp; m; m &= m - 1) s.cid[L.row * N + __ffs(m) - 1] = (uint8_t)nc;
+    left &= ~grp;
+  }
+  for (int k = L.lane; k < nc; k += 32) {
+    s.cnt[k] = 0;
+    s.gone[k] = 0;
+  }
+  __syncwarp();
+  // regions and the chains each is vital to
+  const uint32_t touch = nbr4<N>(own, L);  // points next to an own stone
+  int nr = 0;
+  for (uint32_t left = non;; ++nr) {
+    const unsigned lanes = __ballot_sync(FULL, left != 0u);
+    if (!lanes) break;
+    const int src = __ffs(lanes) - 1;
+    const int sx = __shfl_sync(FULL, __ffs(left) - 1, src);
+    const uint32_t grp = flood<N>(L.lane == src ? 1u << sx : 0u, non, L);
+    left &= ~grp;
+    const uint32_t re = grp & e;
+    int v[4] = {0xFF, 0xFF, 0xFF, 0xFF};
+    const unsigned el = __ballot_sync(FULL, re != 0u);
+    // a region without empty points would be opponent chains without liberties: vital to none
+    if (el && !__any_sync(FULL, (re & ~touch) != 0u)) {
+      const int y0 = __ffs(el) - 1;
+      const int x0 = __shfl_sync(FULL, __ffs(re) - 1, y0);
+      for (int d = 0; d < 4; ++d) {  // the distinct chains next to the first empty point
+        const int x = x0 + d4x(d), y = y0 + d4y(d);
+        if (bit_at<N>(own, x, y)) {
+          const int k = s.cid[y * N + x];
+          if (k != v[0] && k != v[1] && k != v[2]) v[d] = k;
+        }
+      }
+      uint32_t mk[4] = {0u, 0u, 0u, 0u};  // those chains' stones in this row
+      for (uint32_t m = own; m; m &= m - 1) {
+        const int x = __ffs(m) - 1, k = s.cid[L.row * N + x];
+#pragma unroll
+        for (int j = 0; j < 4; ++j)
+          if (k == v[j]) mk[j] |= 1u << x;
+      }
+#pragma unroll
+      for (int j = 0; j < 4; ++j)
+        if (v[j] != 0xFF && __any_sync(FULL, (re & ~nbr4<N>(mk[j], L)) != 0u)) v[j] = 0xFF;
+    }
+    if (L.lane == 0) {
+      s.seed[nr] = (int16_t)(src * N + sx);
+#pragma unroll
+      for (int j = 0; j < 4; ++j) {
+        s.vit[nr][j] = (uint8_t)v[j];
+        if (v[j] != 0xFF) s.cnt[v[j]]++;
+      }
+    }
+  }
+  __syncwarp();
+  // the iteration; `live` holds the points of the regions still in R
+  uint32_t live = non;
+  while (true) {
+    bool ch = false;
+    for (int k = L.lane; k < nc; k += 32)
+      if (!s.gone[k] && s.cnt[k] < 2) {
+        s.gone[k] = 1;
+        ch = true;
+      }
+    if (!__any_sync(FULL, ch)) break;
+    __syncwarp();
+    const uint32_t rem = pa_chain_rows<N>(own, s, L, true);
+    const uint32_t drop = flood<N>(nbr4<N>(rem, L) & live, live, L);
+    if (!__any_sync(FULL, drop != 0u)) break;
+    live &= ~drop;
+    s.rows[0][L.lane] = drop;
+    __syncwarp();
+    for (int r = L.lane; r < nr; r += 32) {
+      const int p = s.seed[r];
+      if ((s.rows[0][p / N] >> (p % N)) & 1u)
+        for (int j = 0; j < 4; ++j)
+          if (s.vit[r][j] != 0xFF) atomicAdd(&s.cnt[s.vit[r][j]], -1);
+    }
+    __syncwarp();
+  }
+  alive = pa_chain_rows<N>(own, s, L, false);
+  // area: the regions left in R with a vital chain left in X, grown from their seed points
+  s.rows[0][L.lane] = live;
+  s.rows[1][L.lane] = 0u;
+  __syncwarp();
+  for (int r = L.lane; r < nr; r += 32) {
+    const int p = s.seed[r], y = p / N, x = p % N;
+    bool keep = false;
+    for (int j = 0; j < 4; ++j) keep |= s.vit[r][j] != 0xFF && !s.gone[s.vit[r][j]];
+    if (keep && ((s.rows[0][y] >> x) & 1u)) atomicOr(&s.rows[1][y], 1u << x);
+  }
+  __syncwarp();
+  area = flood<N>(s.rows[1][L.lane], live, L);
+}
+
+// Both colours: alive = pass-alive stones of either colour, area_b / area_w = black's / white's pass-alive area.
+template <int N>
+__device__ __forceinline__ void pass_alive(uint32_t b, uint32_t w, PaScratch<N>& s, const Lane& L, uint32_t& alive,
+                                           uint32_t& area_b, uint32_t& area_w) {
+  uint32_t ab, aw;
+  pass_alive_colour<N>(b, w, s, L, ab, area_b);
+  pass_alive_colour<N>(w, b, s, L, aw, area_w);
+  alive = ab | aw;
+}
+
+template <int N>
+__global__ void __launch_bounds__(PA_WARPS * 32)
+    k_pass_alive(DevState st, uint8_t* __restrict__ alive_out, uint8_t* __restrict__ area_out) {
+  constexpr int P = Geo<N>::P;
+  __shared__ PaScratch<N> s_pa[PA_WARPS];
+  const Lane L = make_lane_single<N>();
+  const int wid = threadIdx.x >> 5;
+  const int g = blockIdx.x * PA_WARPS + wid;
+  if (g >= st.G) return;  // the whole warp
+  uint32_t b, w, alive, ab, aw;
+  load_row<N>(st.cur, g, L.row, L.active, b, w);
+  pass_alive<N>(b, w, s_pa[wid], L, alive, ab, aw);
+  if (L.active) {
+    for (int x = 0; x < N; ++x) {
+      const size_t a = (size_t)g * P + x * N + L.row;
+      if (alive_out) alive_out[a] = (uint8_t)((alive >> x) & 1u);
+      if (area_out) area_out[a] = (uint8_t)(((ab >> x) & 1u) ? S_BLACK : ((aw >> x) & 1u) ? S_WHITE : 0);
+    }
+  }
+}
+
+// ---------------------------------------------------------------------------------------
 // Dead groups and getTrompTaylorScore (board.cc:1954-2071) of every stored position (elfb200_final_status).
 // One warp per game (row per lane, make_lane_single), groups found one at a time by link-masked fills.
 //
@@ -855,7 +1054,7 @@ __global__ void __launch_bounds__(PLAYOUT_WARPS * 32)
 // Without counts no group is dead.  Dead groups are counted for the opponent (S_DEAD in group_stats): every
 // stone takes its (flipped) colour, an empty region the one colour among the stones it touches, else 3 (dame;
 // also every point of the empty board).  score = black points - white points.
-template <int N>
+template <int N, bool PA = false>
 __global__ void __launch_bounds__(32)
     k_final_status(DevState st, const int32_t* __restrict__ counts, int K, double threshold,
                    uint8_t* __restrict__ dead_out, uint8_t* __restrict__ terr_out, int32_t* __restrict__ score_out) {
@@ -893,6 +1092,12 @@ __global__ void __launch_bounds__(32)
       if ((double)own < -threshold * (double)K * (double)size) dead |= grp;
       left &= ~grp;
     }
+  }
+  if constexpr (PA) {  // pass-alive stones are never dead; the opponent's stones in a pass-alive area always are
+    __shared__ PaScratch<N> s_pa;
+    uint32_t alive, ab, aw;
+    pass_alive<N>(b, w, s_pa, L, alive, ab, aw);
+    dead = (dead & ~alive) | (ab & w) | (aw & b);
   }
   const uint32_t bf = (b & ~dead) | (w & dead), wf = (w & ~dead) | (b & dead);
   const uint32_t e = ~(bf | wf) & L.rm;
@@ -946,18 +1151,6 @@ struct Tac {
   static constexpr int MAX_PATH = 2 * N * N;  // plies of one search
   static constexpr int MAX_PEND = N * N;      // pending branches: capturer nodes are every second ply
 };
-
-// delta4 (board.h:220): (x-1, y), (x, y-1), (x+1, y), (x, y+1)
-__device__ __forceinline__ int d4x(int d) { return d == 0 ? -1 : d == 2 ? 1 : 0; }
-__device__ __forceinline__ int d4y(int d) { return d == 1 ? -1 : d == 3 ? 1 : 0; }
-
-// Point (x, y) of the row words v, false off the board.  Warp-uniform: every lane gets row y by a shuffle.
-template <int N>
-__device__ __forceinline__ bool bit_at(uint32_t v, int x, int y) {
-  const bool on = x >= 0 && x < N && y >= 0 && y < N;
-  const uint32_t r = __shfl_sync(FULL, v, on ? y : 0);
-  return on && ((r >> x) & 1u);
-}
 
 // Sum over the game's rows, the same on every lane of the warp (one game per warp, idle lanes add 0).
 __device__ __forceinline__ int warp_rows_sum(int v, const Lane& L) { return __reduce_add_sync(FULL, L.active ? v : 0); }
@@ -1844,8 +2037,11 @@ int elfb200_ownership(elfb200_ctx* c, int playouts, uint64_t seed, int max_plies
   return ELFB200_OK;
 }
 
-int elfb200_final_status(elfb200_ctx* c, const int32_t* counts_host, int playouts, double threshold,
-                         uint8_t* dead_host, uint8_t* territory_host, int32_t* score_host) {
+}  // extern "C"
+
+// elfb200_final_status and, with pa, elfb200_final_status_pass_alive (k_final_status<N, true>)
+static int final_status_run(elfb200_ctx* c, const int32_t* counts_host, int playouts, double threshold,
+                            uint8_t* dead_host, uint8_t* territory_host, int32_t* score_host, bool pa) {
   if (!c) return elfb200_fail(ELFB200_ERR_ARG, "ctx is NULL");
   if (counts_host && playouts < 1)
     return elfb200_fail(ELFB200_ERR_ARG, "playouts must be at least 1 (got %d)", playouts);
@@ -1863,15 +2059,71 @@ int elfb200_final_status(elfb200_ctx* c, const int32_t* counts_host, int playout
   }
   uint8_t* ddead = c->d_own_status;
   uint8_t* dterr = c->d_own_status + G * P;
-  DISPATCH_N(c, (k_final_status<19><<<c->G, 32, 0, c->stream>>>(c->st, dcounts, playouts, threshold, ddead, dterr,
-                                                                c->d_words)),
-             (k_final_status<9><<<c->G, 32, 0, c->stream>>>(c->st, dcounts, playouts, threshold, ddead, dterr,
-                                                               c->d_words)));
+  if (pa)
+    DISPATCH_N(c, (k_final_status<19, true><<<c->G, 32, 0, c->stream>>>(c->st, dcounts, playouts, threshold, ddead,
+                                                                         dterr, c->d_words)),
+               (k_final_status<9, true><<<c->G, 32, 0, c->stream>>>(c->st, dcounts, playouts, threshold, ddead, dterr,
+                                                                       c->d_words)));
+  else
+    DISPATCH_N(c, (k_final_status<19><<<c->G, 32, 0, c->stream>>>(c->st, dcounts, playouts, threshold, ddead, dterr,
+                                                                  c->d_words)),
+               (k_final_status<9><<<c->G, 32, 0, c->stream>>>(c->st, dcounts, playouts, threshold, ddead, dterr,
+                                                                 c->d_words)));
   c->launches++;
   CK(cudaGetLastError());
   if (dead_host) CK(cudaMemcpyAsync(dead_host, ddead, G * P, cudaMemcpyDeviceToHost, c->stream));
   if (territory_host) CK(cudaMemcpyAsync(territory_host, dterr, G * P, cudaMemcpyDeviceToHost, c->stream));
   if (score_host) CK(cudaMemcpyAsync(score_host, c->d_words, G * sizeof(int32_t), cudaMemcpyDeviceToHost, c->stream));
+  CK(cudaStreamSynchronize(c->stream));
+  return ELFB200_OK;
+}
+
+extern "C" {
+
+int elfb200_final_status(elfb200_ctx* c, const int32_t* counts_host, int playouts, double threshold,
+                         uint8_t* dead_host, uint8_t* territory_host, int32_t* score_host) {
+  return final_status_run(c, counts_host, playouts, threshold, dead_host, territory_host, score_host, false);
+}
+
+int elfb200_final_status_pass_alive(elfb200_ctx* c, const int32_t* counts_host, int playouts, double threshold,
+                                    uint8_t* dead_host, uint8_t* territory_host, int32_t* score_host) {
+  return final_status_run(c, counts_host, playouts, threshold, dead_host, territory_host, score_host, true);
+}
+
+}  // extern "C"
+
+// ---- pass-alive chains and areas ---------------------------------------------------------------------------------
+static int pass_alive_launch(elfb200_ctx* c, uint8_t* alive, uint8_t* area) {
+  const int grid = (c->G + PA_WARPS - 1) / PA_WARPS;
+  DISPATCH_N(c, (k_pass_alive<19><<<grid, PA_WARPS * 32, 0, c->stream>>>(c->st, alive, area)),
+             (k_pass_alive<9><<<grid, PA_WARPS * 32, 0, c->stream>>>(c->st, alive, area)));
+  c->launches++;
+  CK(cudaGetLastError());
+  return ELFB200_OK;
+}
+
+extern "C" {
+
+int elfb200_pass_alive_dev(elfb200_ctx* c, uint8_t* alive_dev, uint8_t* area_dev) {
+  if (!c) return elfb200_fail(ELFB200_ERR_ARG, "ctx is NULL");
+  if (!alive_dev && !area_dev) return ELFB200_OK;
+  CK(cudaSetDevice(c->device));
+  return pass_alive_launch(c, alive_dev, area_dev);
+}
+
+int elfb200_pass_alive(elfb200_ctx* c, uint8_t* alive_host, uint8_t* area_host) {
+  if (!c) return elfb200_fail(ELFB200_ERR_ARG, "ctx is NULL");
+  if (!alive_host && !area_host) return ELFB200_OK;
+  CK(cudaSetDevice(c->device));
+  const size_t n = (size_t)c->G * c->N * c->N;
+  // final status's buffer (G * 2 * N*N bytes): both calls are synchronous
+  if (!c->d_own_status) CK(cudaMalloc(&c->d_own_status, 2 * n));
+  uint8_t* da = alive_host ? c->d_own_status : nullptr;
+  uint8_t* dr = area_host ? c->d_own_status + n : nullptr;
+  int rc = pass_alive_launch(c, da, dr);
+  if (rc) return rc;
+  if (da) CK(cudaMemcpyAsync(alive_host, da, n, cudaMemcpyDeviceToHost, c->stream));
+  if (dr) CK(cudaMemcpyAsync(area_host, dr, n, cudaMemcpyDeviceToHost, c->stream));
   CK(cudaStreamSynchronize(c->stream));
   return ELFB200_OK;
 }

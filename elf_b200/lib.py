@@ -65,6 +65,9 @@ SIGNATURES = {
     "elfb200_final_status": (ctypes.c_int, [vp, vp, ctypes.c_int, ctypes.c_double, vp, vp, vp]),
     "elfb200_tactics": (ctypes.c_int, [vp, vp, vp, vp]),
     "elfb200_tactics_dev": (ctypes.c_int, [vp, vp, vp]),
+    "elfb200_pass_alive": (ctypes.c_int, [vp, vp, vp]),
+    "elfb200_pass_alive_dev": (ctypes.c_int, [vp, vp, vp]),
+    "elfb200_final_status_pass_alive": (ctypes.c_int, [vp, vp, ctypes.c_int, ctypes.c_double, vp, vp, vp]),
     "elfb200_playout_stream": (ctypes.c_int, [vp, ctypes.c_uint64, ctypes.c_uint64, ctypes.c_int, vp, vp, vp, vp, vp]),
     "elfb200_playout_stream_launch": (ctypes.c_int, [vp, ctypes.c_uint64, ctypes.c_uint64, ctypes.c_int]),
     # include/elfb200_mcts.h

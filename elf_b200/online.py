@@ -258,11 +258,13 @@ class OnlineGame:
         self._final_kept = True
 
     # -- end of game: dead stones -------------------------------------------------------------------
-    def final_status(self, playouts=1024, seed=0, threshold=0.5):
+    def final_status(self, playouts=1024, seed=0, threshold=0.5, pass_alive=False):
         """dead and alive groups of the position the game ended in: the kept final position when the board
         was restarted after a finished game and nothing has been played since, the current position otherwise.
         A group is dead when ``playouts`` random playouts from the position leave its stones, on average, more
-        than ``threshold`` in the opponent's area (``GoBatch.ownership`` / ``GoBatch.final_status``).  Returns
+        than ``threshold`` in the opponent's area (``GoBatch.ownership`` / ``GoBatch.final_status``).
+        ``pass_alive=True`` adds Benson's exact rule (``GoBatch.final_status(pass_alive=True)``): pass-alive
+        groups are never dead, and opponent stones inside a pass-alive area always are.  Returns
         ``(dead, alive)``: lists of groups, each a list of actions (x*N+y) in ascending order, the groups
         ordered by their lowest action."""
         board = self.board
@@ -270,7 +272,10 @@ class OnlineGame:
         if self._final_kept and int(i[0]) == 1 and not board.stones()[0].any():
             board = self._final
         counts = board.ownership(playouts, seed=seed)
-        dead = board.final_status(counts, playouts, threshold)[0][0]
+        if pass_alive:
+            dead = board.final_status(counts, playouts, threshold, pass_alive=True)[0][0]
+        else:
+            dead = board.final_status(counts, playouts, threshold)[0][0]
         dead_groups, alive_groups = [], []
         for grp in stone_groups(board.stones()[0], self.N):
             (dead_groups if dead[grp[0]] else alive_groups).append(grp)

@@ -219,6 +219,29 @@ int elfb200_tactics(elfb200_ctx* ctx, int16_t* ladder_host, int16_t* self_atari_
  * stream.  Needs no scratch: capturable in a CUDA graph from the first call. */
 int elfb200_tactics_dev(elfb200_ctx* ctx, int16_t* ladder_dev, int16_t* self_atari_dev);
 
+/* Pass-alive chains and areas of the stored positions, both colours (Benson's unconditional life; the reference
+ * has no counterpart).  For a colour c, a chain is a maximal 4-connected set of c stones and a region a maximal
+ * 4-connected set of points that hold no c stone; a region is vital to a chain when every empty point of the
+ * region is a liberty of the chain.  Starting from every chain in X and every region in R, repeat until nothing
+ * changes: remove from X every chain with fewer than two regions of R vital to it, then remove from R every
+ * region that borders a chain no longer in X.  The stones of the chains left in X are pass-alive: they cannot be
+ * captured even if c passes forever.  c's pass-alive area is every point (empty, or an opponent stone) of a region
+ * left in R that is vital to a chain left in X; opponent stones there are dead with certainty.  Only the position
+ * is read (not the history, the ko point or the side to move).  alive uint8 [G][N*N] by action x*N+y: 1 on every
+ * stone of a pass-alive chain of either colour (the stone's colour says whose); area uint8 [G][N*N]: 1 in black's
+ * pass-alive area, 2 in white's, 0 elsewhere.  Either output may be NULL and its work is skipped.  The stored
+ * games are not changed.  Synchronous. */
+int elfb200_pass_alive(elfb200_ctx* ctx, uint8_t* alive_host, uint8_t* area_host);
+/* The same into device memory (either may be NULL), asynchronous on the context stream.  Needs no scratch:
+ * capturable in a CUDA graph from the first call. */
+int elfb200_pass_alive_dev(elfb200_ctx* ctx, uint8_t* alive_dev, uint8_t* area_dev);
+/* elfb200_final_status with the pass-alive rule: dead = (the stones elfb200_final_status's playout rule finds dead,
+ * minus pass-alive stones) + (opponent stones inside a pass-alive area).  With counts_host == NULL only the second
+ * part applies: an exact, playout-free dead-stone rule.  Arguments, outputs, territory and score as in
+ * elfb200_final_status. */
+int elfb200_final_status_pass_alive(elfb200_ctx* ctx, const int32_t* counts_host, int playouts, double threshold,
+                                    uint8_t* dead_host, uint8_t* territory_host, int32_t* score_host);
+
 /* Number of kernels this library has launched since creation (bench gpu_launches).  Counts enqueues by
  * the calls above; replays of a CUDA graph that captured them are not counted. */
 int64_t elfb200_launch_count(const elfb200_ctx* ctx);

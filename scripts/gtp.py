@@ -31,6 +31,8 @@ def main():
     ap.add_argument("--device", type=int, default=0)
     ap.add_argument("--use-df-feature", action="store_true",
                     help="a DarkForest-plane network (GameOptions::use_df_feature): 25 input planes")
+    ap.add_argument("--pass-alive", action="store_true",
+                    help="final_status_list: pass-alive groups are never dead, opponent stones in their area always are")
     args = ap.parse_args()
 
     import torch
@@ -54,7 +56,9 @@ def main():
         preload_sgf=args.preload_sgf, preload_sgf_move_to=args.preload_sgf_move_to, num_rollouts=args.rollouts,
         num_rollouts_per_batch=args.per_batch, c_puct=args.puct, virtual_loss=args.virtual_loss, persistent_tree=1,
         rotation_flip=1, use_df_feature=args.use_df_feature)
-    GtpConsole(game, actor).run()
+    console = GtpConsole(game, actor)
+    console.final_status_pass_alive = args.pass_alive
+    console.run()
 
 
 if __name__ == "__main__":
