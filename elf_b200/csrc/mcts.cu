@@ -1158,10 +1158,10 @@ __device__ __forceinline__ float rng_u01(uint64_t key, uint32_t& ctr);  // defin
 // The uniform comes from a counter-based generator (seed, game, ply): same distribution as the
 // reference's per-game mt19937, different stream.  One warp per game.
 template <int N>
-__global__ void __launch_bounds__(BLOCK)
-    k_choose(DevState st, TreeDev tr, int cutoff, float resign_thres, const uint8_t* __restrict__ never_resign,
-             uint64_t seed, int32_t* __restrict__ action_out, float* __restrict__ value_out) {
-  __shared__ OrderScratch scratch[BLOCK / 32];
+__device__ __forceinline__ void choose_game(const DevState& st, const TreeDev& tr, int cutoff, float resign_thres,
+                                            const uint8_t* __restrict__ never_resign, uint64_t seed,
+                                            int32_t* __restrict__ action_out, float* __restrict__ value_out,
+                                            OrderScratch* scratch) {
   const int lane = threadIdx.x & 31;
   const int g = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
   if (g >= st.G) return;
@@ -1218,6 +1218,24 @@ __global__ void __launch_bounds__(BLOCK)
     action_out[g] = a;
     if (value_out) value_out[g] = q;
   }
+}
+
+template <int N>
+__global__ void __launch_bounds__(BLOCK)
+    k_choose(DevState st, TreeDev tr, int cutoff, float resign_thres, const uint8_t* __restrict__ never_resign,
+             uint64_t seed, int32_t* __restrict__ action_out, float* __restrict__ value_out) {
+  __shared__ OrderScratch scratch[BLOCK / 32];
+  choose_game<N>(st, tr, cutoff, resign_thres, never_resign, seed, action_out, value_out, scratch);
+}
+
+// elfb200_mcts_choose_dev: the seed read from device memory, so that a graph replay draws with the seed the
+// caller's device counter holds at that point, not the value it had when the graph was captured.
+template <int N>
+__global__ void __launch_bounds__(BLOCK)
+    k_choose(DevState st, TreeDev tr, int cutoff, float resign_thres, const uint8_t* __restrict__ never_resign,
+             const int64_t* __restrict__ seed, int32_t* __restrict__ action_out, float* __restrict__ value_out) {
+  __shared__ OrderScratch scratch[BLOCK / 32];
+  choose_game<N>(st, tr, cutoff, resign_thres, never_resign, (uint64_t)*seed, action_out, value_out, scratch);
 }
 
 // ---------------------------------------------------------------------------------------
@@ -1333,8 +1351,8 @@ __device__ __forceinline__ float rng_gamma(float a, uint64_t key, uint32_t& ctr)
   return d * boost;
 }
 
-__global__ void __launch_bounds__(BLOCK)
-    k_root_noise(int G, TreeDev tr, float eps, float alpha, uint64_t seed, uint32_t move_counter) {
+__device__ __forceinline__ void root_noise(int G, const TreeDev& tr, float eps, float alpha, uint64_t seed,
+                                           uint32_t move_counter) {
   const int lane = threadIdx.x & 31;
   const int g = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
   if (g >= G || !tr.active[g]) return;
@@ -1361,6 +1379,18 @@ __global__ void __launch_bounds__(BLOCK)
     es[i].x = (1.f - eps) * es[i].x + eps * eta / z;
   }
   if (lane == 0) tr.hdr[nb + root].flags |= NF_FULLSCAN;
+}
+
+__global__ void __launch_bounds__(BLOCK)
+    k_root_noise(int G, TreeDev tr, float eps, float alpha, uint64_t seed, uint32_t move_counter) {
+  root_noise(G, tr, eps, alpha, seed, move_counter);
+}
+
+// elfb200_mcts_begin_move_dev: the move index read from device memory, so that every replay of a captured move
+// draws the noise of the move the caller's counter holds, as the host form draws that of its host counter.
+__global__ void __launch_bounds__(BLOCK)
+    k_root_noise(int G, TreeDev tr, float eps, float alpha, uint64_t seed, const int64_t* __restrict__ move) {
+  root_noise(G, tr, eps, alpha, seed, (uint32_t)*move);
 }
 
 __global__ void __launch_bounds__(BLOCK) k_root_priors(int G, TreeDev tr, float* __restrict__ out, int P1) {
@@ -1783,6 +1813,50 @@ int elfb200_mcts_waves_per_move(const elfb200_mcts* m) { return m ? m->waves_per
 int elfb200_mcts_max_leaves(const elfb200_mcts* m) { return m ? m->ctx->G * m->tr.B : 0; }
 int elfb200_mcts_nodes_per_game(const elfb200_mcts* m) { return m ? m->tr.C : 0; }
 
+// ---- one launch function per operation, shared by the host form and the device form (_dev) ----------------------
+// The device forms pass device pointers, skip the timing events and never wait for the stream, so that they can be
+// captured in a CUDA graph; everything they launch is what the host forms launch.
+
+// The device forms are refused while a reference D4 stream is set: that stream is refilled from the host every move.
+static int check_dev_form(const elfb200_mcts* m) {
+  if (!m) return elfb200_fail(ELFB200_ERR_ARG, "mcts is NULL");
+  if (m->tr.d4_stream)
+    return elfb200_fail(ELFB200_ERR_STATE, "a reference D4 stream is set (elfb200_mcts_set_d4_stream): it is fed "
+                                           "from the host every move, so the device forms are not available");
+  return ELFB200_OK;
+}
+
+static int tree_reset_launch(elfb200_mcts* m, const uint8_t* mask_dev) {
+  elfb200_ctx* c = m->ctx;
+  k_tree_reset<<<warp_grid(c->G), BLOCK, 0, c->stream>>>(c->G, m->tr, mask_dev);
+  c->launches++;
+  CK(cudaGetLastError());
+  return ELFB200_OK;
+}
+
+// k_begin and the root noise, keyed by the host counter (move_dev NULL) or by the move index in device memory
+static int begin_move_launch(elfb200_mcts* m, const int64_t* move_dev) {
+  elfb200_ctx* c = m->ctx;
+  const int need = m->waves_per_move * m->tr.B;
+  DISPATCH_N(c, (k_begin<19><<<warp_grid(c->G), BLOCK, 0, c->stream>>>(c->st, m->tr, need)),
+             (k_begin<9><<<warp_grid(c->G), BLOCK, 0, c->stream>>>(c->st, m->tr, need)));
+  c->launches++;
+  CK(cudaGetLastError());
+  if (m->opt.root_epsilon > 0.f) {
+    const uint64_t seed = (uint64_t)(uint32_t)m->opt.seed;
+    if (move_dev)
+      k_root_noise<<<warp_grid(c->G), BLOCK, 0, c->stream>>>(c->G, m->tr, m->opt.root_epsilon, m->opt.root_alpha,
+                                                              seed, move_dev);
+    else
+      k_root_noise<<<warp_grid(c->G), BLOCK, 0, c->stream>>>(c->G, m->tr, m->opt.root_epsilon, m->opt.root_alpha,
+                                                              seed, m->move_counter);
+    c->launches++;
+    CK(cudaGetLastError());
+  }
+  m->wave = 0;
+  return ELFB200_OK;
+}
+
 int elfb200_mcts_reset(elfb200_mcts* m, const uint8_t* mask_host) {
   if (!m) return elfb200_fail(ELFB200_ERR_ARG, "mcts is NULL");
   elfb200_ctx* c = m->ctx;
@@ -1793,11 +1867,17 @@ int elfb200_mcts_reset(elfb200_mcts* m, const uint8_t* mask_host) {
     CK(cudaMemcpyAsync(m->d_mask, c->h_pin, c->G, cudaMemcpyHostToDevice, c->stream));
     dm = m->d_mask;
   }
-  k_tree_reset<<<warp_grid(c->G), BLOCK, 0, c->stream>>>(c->G, m->tr, dm);
-  c->launches++;
-  CK(cudaGetLastError());
+  const int rc = tree_reset_launch(m, dm);
+  if (rc) return rc;
   CK(cudaStreamSynchronize(c->stream));
   return ELFB200_OK;
+}
+
+int elfb200_mcts_reset_dev(elfb200_mcts* m, const uint8_t* mask_dev) {
+  const int rc = check_dev_form(m);
+  if (rc) return rc;
+  CK(cudaSetDevice(m->ctx->device));
+  return tree_reset_launch(m, mask_dev);
 }
 
 int elfb200_mcts_begin_move(elfb200_mcts* m, const uint8_t* active_host) {
@@ -1810,42 +1890,47 @@ int elfb200_mcts_begin_move(elfb200_mcts* m, const uint8_t* active_host) {
   } else {
     CK(cudaMemsetAsync(m->tr.active, 1, c->G, c->stream));
   }
-  const int need = m->waves_per_move * m->tr.B;
-  DISPATCH_N(c, (k_begin<19><<<warp_grid(c->G), BLOCK, 0, c->stream>>>(c->st, m->tr, need)),
-             (k_begin<9><<<warp_grid(c->G), BLOCK, 0, c->stream>>>(c->st, m->tr, need)));
-  c->launches++;
-  CK(cudaGetLastError());
-  if (m->opt.root_epsilon > 0.f) {
-    k_root_noise<<<warp_grid(c->G), BLOCK, 0, c->stream>>>(c->G, m->tr, m->opt.root_epsilon, m->opt.root_alpha,
-                                                            (uint64_t)(uint32_t)m->opt.seed, m->move_counter);
-    c->launches++;
-    CK(cudaGetLastError());
-  }
+  const int rc = begin_move_launch(m, nullptr);
+  if (rc) return rc;
   m->move_counter++;
-  m->wave = 0;
   return ELFB200_OK;
 }
 
-int elfb200_mcts_select_ex(elfb200_mcts* m, void* feat_dev, int format, int cpad, int32_t* n_leaves) {
-  if (!m || !feat_dev) return elfb200_fail(ELFB200_ERR_ARG, "NULL argument");
-  elfb200_ctx* c = m->ctx;
-  const int rc = check_leaf_format(feat_dev, format, cpad);
+int elfb200_mcts_begin_move_dev(elfb200_mcts* m, const uint8_t* active_dev, const int64_t* move_dev) {
+  int rc = check_dev_form(m);
   if (rc) return rc;
+  if (!move_dev && m->opt.root_epsilon > 0.f)
+    return elfb200_fail(ELFB200_ERR_ARG, "move_dev is NULL with root noise on (root_epsilon > 0)");
+  if (m->wave_open) return elfb200_fail(ELFB200_ERR_STATE, "a wave is open (select without expand_backup)");
+  elfb200_ctx* c = m->ctx;
   CK(cudaSetDevice(c->device));
-  if (m->pending_sel || m->pending_feat || m->pending_eb) {
+  if (active_dev)
+    CK(cudaMemcpyAsync(m->tr.active, active_dev, c->G, cudaMemcpyDeviceToDevice, c->stream));
+  else
+    CK(cudaMemsetAsync(m->tr.active, 1, c->G, c->stream));
+  return begin_move_launch(m, move_dev);
+}
+
+// One wave's descents and leaf planes.  timed: the host form's event pairs around the kernels (and the wait
+// for the previous wave's, which the pairs are reused from); n_leaves as in elfb200_mcts_select_ex.
+static int select_launch(elfb200_mcts* m, void* feat_dev, int format, int cpad, int32_t* n_leaves, bool timed) {
+  elfb200_ctx* c = m->ctx;
+  if (timed && (m->pending_sel || m->pending_feat || m->pending_eb)) {
     // the event pairs are reused every wave: read the previous wave's before re-recording them
     // (only reached in the asynchronous mode; the synchronous mode flushed after its own sync)
     CK(cudaEventSynchronize(m->ev[6]));
     flush_timings(m);
   }
   CK(cudaMemsetAsync(m->tr.eval_count, 0, 4, c->stream));
-  CK(cudaEventRecord(m->ev[0], c->stream));
+  if (timed) CK(cudaEventRecord(m->ev[0], c->stream));
   DISPATCH_N(c, (k_select<19><<<warp_grid(c->G), BLOCK, 0, c->stream>>>(c->st, m->tr, m->so, m->wave)),
              (k_select<9><<<warp_grid(c->G), BLOCK, 0, c->stream>>>(c->st, m->tr, m->so, m->wave)));
   c->launches++;
   CK(cudaGetLastError());
-  CK(cudaEventRecord(m->ev[1], c->stream));
-  m->pending_sel = true;
+  if (timed) {
+    CK(cudaEventRecord(m->ev[1], c->stream));
+    m->pending_sel = true;
+  }
   m->wave_open = true;
   int n = -1;  // unknown to the host: the feature / expand grids cover all G*B slots and the kernels
                // stop at the device-side count
@@ -1863,14 +1948,35 @@ int elfb200_mcts_select_ex(elfb200_mcts* m, void* feat_dev, int format, int cpad
   m->last_eval_count = n;
   if (n != 0) {
     const int npos = n > 0 ? n : c->G * m->tr.B;
-    CK(cudaEventRecord(m->ev[2], c->stream));
+    if (timed) CK(cudaEventRecord(m->ev[2], c->stream));
     launch_leaf_features(m, feat_dev, format, cpad, npos);
     CK(cudaGetLastError());
-    CK(cudaEventRecord(m->ev[3], c->stream));
-    m->pending_feat = true;
+    if (timed) {
+      CK(cudaEventRecord(m->ev[3], c->stream));
+      m->pending_feat = true;
+    }
   }
   m->wave++;
   return ELFB200_OK;
+}
+
+int elfb200_mcts_select_ex(elfb200_mcts* m, void* feat_dev, int format, int cpad, int32_t* n_leaves) {
+  if (!m || !feat_dev) return elfb200_fail(ELFB200_ERR_ARG, "NULL argument");
+  const int rc = check_leaf_format(feat_dev, format, cpad);
+  if (rc) return rc;
+  CK(cudaSetDevice(m->ctx->device));
+  return select_launch(m, feat_dev, format, cpad, n_leaves, true);
+}
+
+int elfb200_mcts_select_dev(elfb200_mcts* m, void* feat_dev, int format, int cpad) {
+  int rc = check_dev_form(m);
+  if (rc) return rc;
+  if (!feat_dev) return elfb200_fail(ELFB200_ERR_ARG, "feat_dev is NULL");
+  rc = check_leaf_format(feat_dev, format, cpad);
+  if (rc) return rc;
+  if (m->wave_open) return elfb200_fail(ELFB200_ERR_STATE, "a wave is open (select without expand_backup)");
+  CK(cudaSetDevice(m->ctx->device));
+  return select_launch(m, feat_dev, format, cpad, nullptr, false);
 }
 
 int elfb200_mcts_leaf_features(elfb200_mcts* m, void* feat_dev, int format, int cpad) {
@@ -1923,12 +2029,11 @@ int elfb200_mcts_leaf_info(elfb200_mcts* m, uint64_t* hash_host, int32_t* game_h
   return ELFB200_OK;
 }
 
-int elfb200_mcts_expand_backup(elfb200_mcts* m, const float* pi_dev, const float* value_dev) {
-  if (!m) return elfb200_fail(ELFB200_ERR_ARG, "mcts is NULL");
+// Expansion with the network's reply, then backup; timed as in select_launch.
+static int expand_backup_launch(elfb200_mcts* m, const float* pi_dev, const float* value_dev, bool timed) {
   elfb200_ctx* c = m->ctx;
-  CK(cudaSetDevice(c->device));
   const int n = m->last_eval_count;
-  CK(cudaEventRecord(m->ev[4], c->stream));
+  if (timed) CK(cudaEventRecord(m->ev[4], c->stream));
   if (n != 0) {
     if (!pi_dev || !value_dev) return elfb200_fail(ELFB200_ERR_ARG, "pi/value is NULL with %d leaves pending", n);
     const int nw = n > 0 ? n : c->G * m->tr.B;  // n < 0: count known to the device only
@@ -1941,13 +2046,40 @@ int elfb200_mcts_expand_backup(elfb200_mcts* m, const float* pi_dev, const float
     c->launches++;
     CK(cudaGetLastError());
   }
-  CK(cudaEventRecord(m->ev[5], c->stream));
+  if (timed) CK(cudaEventRecord(m->ev[5], c->stream));
   k_backup<<<warp_grid(c->G), BLOCK, 0, c->stream>>>(c->G, m->tr, m->so.virtual_loss);
   c->launches++;
   CK(cudaGetLastError());
-  CK(cudaEventRecord(m->ev[6], c->stream));
-  m->pending_eb = true;
+  if (timed) {
+    CK(cudaEventRecord(m->ev[6], c->stream));
+    m->pending_eb = true;
+  }
   m->wave_open = false;
+  return ELFB200_OK;
+}
+
+int elfb200_mcts_expand_backup(elfb200_mcts* m, const float* pi_dev, const float* value_dev) {
+  if (!m) return elfb200_fail(ELFB200_ERR_ARG, "mcts is NULL");
+  CK(cudaSetDevice(m->ctx->device));
+  return expand_backup_launch(m, pi_dev, value_dev, true);
+}
+
+int elfb200_mcts_expand_backup_dev(elfb200_mcts* m, const float* pi_dev, const float* value_dev) {
+  const int rc = check_dev_form(m);
+  if (rc) return rc;
+  if (!pi_dev || !value_dev) return elfb200_fail(ELFB200_ERR_ARG, "pi/value is NULL");
+  if (!m->wave_open) return elfb200_fail(ELFB200_ERR_STATE, "no wave is open (expand_backup without select)");
+  CK(cudaSetDevice(m->ctx->device));
+  return expand_backup_launch(m, pi_dev, value_dev, false);
+}
+
+// k_results into the given device tables (each may be NULL)
+static int results_launch(elfb200_mcts* m, int32_t* best, int32_t* visits, float* rootv, float* bestq, int32_t* total) {
+  elfb200_ctx* c = m->ctx;
+  DISPATCH_N(c, (k_results<19><<<warp_grid(c->G), BLOCK, 0, c->stream>>>(c->G, m->tr, best, visits, rootv, bestq, total)),
+             (k_results<9><<<warp_grid(c->G), BLOCK, 0, c->stream>>>(c->G, m->tr, best, visits, rootv, bestq, total)));
+  c->launches++;
+  CK(cudaGetLastError());
   return ELFB200_OK;
 }
 
@@ -1957,13 +2089,8 @@ int elfb200_mcts_results(elfb200_mcts* m, int32_t* best_action_host, int32_t* vi
   elfb200_ctx* c = m->ctx;
   CK(cudaSetDevice(c->device));
   const size_t G = c->G, P1 = (size_t)c->N * c->N + 1;
-  DISPATCH_N(c,
-             (k_results<19><<<warp_grid(c->G), BLOCK, 0, c->stream>>>(c->G, m->tr, m->d_best, m->d_visits,
-                                                                       m->d_rootv, m->d_bestq, m->d_total)),
-             (k_results<9><<<warp_grid(c->G), BLOCK, 0, c->stream>>>(c->G, m->tr, m->d_best, m->d_visits,
-                                                                      m->d_rootv, m->d_bestq, m->d_total)));
-  c->launches++;
-  CK(cudaGetLastError());
+  const int rc = results_launch(m, m->d_best, m->d_visits, m->d_rootv, m->d_bestq, m->d_total);
+  if (rc) return rc;
   if (best_action_host) CK(cudaMemcpyAsync(best_action_host, m->d_best, G * 4, cudaMemcpyDeviceToHost, c->stream));
   if (visits_host) CK(cudaMemcpyAsync(visits_host, m->d_visits, G * P1 * 4, cudaMemcpyDeviceToHost, c->stream));
   if (root_value_host) CK(cudaMemcpyAsync(root_value_host, m->d_rootv, G * 4, cudaMemcpyDeviceToHost, c->stream));
@@ -1973,16 +2100,52 @@ int elfb200_mcts_results(elfb200_mcts* m, int32_t* best_action_host, int32_t* vi
   return ELFB200_OK;
 }
 
+static int advance_launch(elfb200_mcts* m, const int32_t* actions_dev) {
+  elfb200_ctx* c = m->ctx;
+  k_advance<<<warp_grid(c->G), BLOCK, 0, c->stream>>>(c->G, m->tr, actions_dev, m->so.persistent);
+  c->launches++;
+  CK(cudaGetLastError());
+  return ELFB200_OK;
+}
+
 int elfb200_mcts_advance(elfb200_mcts* m, const int32_t* actions_host) {
   if (!m || !actions_host) return elfb200_fail(ELFB200_ERR_ARG, "NULL argument");
   elfb200_ctx* c = m->ctx;
   CK(cudaSetDevice(c->device));
   memcpy(c->h_pin, actions_host, (size_t)c->G * 4);
   CK(cudaMemcpyAsync(m->d_actions, c->h_pin, (size_t)c->G * 4, cudaMemcpyHostToDevice, c->stream));
-  k_advance<<<warp_grid(c->G), BLOCK, 0, c->stream>>>(c->G, m->tr, m->d_actions, m->so.persistent);
+  const int rc = advance_launch(m, m->d_actions);
+  if (rc) return rc;
+  CK(cudaStreamSynchronize(c->stream));
+  return ELFB200_OK;
+}
+
+int elfb200_mcts_advance_dev(elfb200_mcts* m, const int32_t* actions_dev) {
+  const int rc = check_dev_form(m);
+  if (rc) return rc;
+  if (!actions_dev) return elfb200_fail(ELFB200_ERR_ARG, "actions_dev is NULL");
+  CK(cudaSetDevice(m->ctx->device));
+  return advance_launch(m, actions_dev);
+}
+
+// k_choose with the seed by value (seed_dev NULL) or read from device memory
+static int choose_launch(elfb200_mcts* m, int cutoff, float resign_thres, const uint8_t* never_resign_dev,
+                         uint64_t seed, const int64_t* seed_dev, int32_t* actions_dev, float* values_dev) {
+  elfb200_ctx* c = m->ctx;
+  if (seed_dev)
+    DISPATCH_N(c,
+               (k_choose<19><<<warp_grid(c->G), BLOCK, 0, c->stream>>>(c->st, m->tr, cutoff, resign_thres,
+                                                                        never_resign_dev, seed_dev, actions_dev, values_dev)),
+               (k_choose<9><<<warp_grid(c->G), BLOCK, 0, c->stream>>>(c->st, m->tr, cutoff, resign_thres,
+                                                                       never_resign_dev, seed_dev, actions_dev, values_dev)));
+  else
+    DISPATCH_N(c,
+               (k_choose<19><<<warp_grid(c->G), BLOCK, 0, c->stream>>>(c->st, m->tr, cutoff, resign_thres,
+                                                                        never_resign_dev, seed, actions_dev, values_dev)),
+               (k_choose<9><<<warp_grid(c->G), BLOCK, 0, c->stream>>>(c->st, m->tr, cutoff, resign_thres,
+                                                                       never_resign_dev, seed, actions_dev, values_dev)));
   c->launches++;
   CK(cudaGetLastError());
-  CK(cudaStreamSynchronize(c->stream));
   return ELFB200_OK;
 }
 
@@ -1999,17 +2162,30 @@ int elfb200_mcts_choose(elfb200_mcts* m, int policy_distri_cutoff, float resign_
     CK(cudaMemcpyAsync(m->d_mask, c->h_pin, G, cudaMemcpyHostToDevice, c->stream));
     nr = m->d_mask;
   }
-  DISPATCH_N(c,
-             (k_choose<19><<<warp_grid(c->G), BLOCK, 0, c->stream>>>(c->st, m->tr, policy_distri_cutoff, resign_thres,
-                                                                      nr, seed, m->d_best, m->d_bestq)),
-             (k_choose<9><<<warp_grid(c->G), BLOCK, 0, c->stream>>>(c->st, m->tr, policy_distri_cutoff, resign_thres,
-                                                                     nr, seed, m->d_best, m->d_bestq)));
-  c->launches++;
-  CK(cudaGetLastError());
+  const int rc = choose_launch(m, policy_distri_cutoff, resign_thres, nr, seed, nullptr, m->d_best, m->d_bestq);
+  if (rc) return rc;
   CK(cudaMemcpyAsync(actions_host, m->d_best, G * 4, cudaMemcpyDeviceToHost, c->stream));
   if (values_host) CK(cudaMemcpyAsync(values_host, m->d_bestq, G * 4, cudaMemcpyDeviceToHost, c->stream));
   CK(cudaStreamSynchronize(c->stream));
   return ELFB200_OK;
+}
+
+int elfb200_mcts_choose_dev(elfb200_mcts* m, int policy_distri_cutoff, float resign_thres,
+                            const uint8_t* never_resign_dev, const int64_t* seed_dev, int32_t* actions_dev,
+                            float* values_dev) {
+  const int rc = check_dev_form(m);
+  if (rc) return rc;
+  if (!seed_dev || !actions_dev) return elfb200_fail(ELFB200_ERR_ARG, "seed_dev/actions_dev is NULL");
+  CK(cudaSetDevice(m->ctx->device));
+  return choose_launch(m, policy_distri_cutoff, resign_thres, never_resign_dev, 0, seed_dev, actions_dev, values_dev);
+}
+
+int elfb200_mcts_results_dev(elfb200_mcts* m, int32_t* best_action_dev, int32_t* visits_dev, float* root_value_dev,
+                             float* best_q_dev, int32_t* total_visits_dev) {
+  const int rc = check_dev_form(m);
+  if (rc) return rc;
+  CK(cudaSetDevice(m->ctx->device));
+  return results_launch(m, best_action_dev, visits_dev, root_value_dev, best_q_dev, total_visits_dev);
 }
 
 int elfb200_mcts_root_priors(elfb200_mcts* m, float* priors_host) {

@@ -110,6 +110,13 @@ SIGNATURES = {
     "elfb200_mcts_gather": (ctypes.c_int, [vp, vp, vp]),
     "elfb200_mcts_gather_dev": (ctypes.c_int, [vp, vp, vp]),
     "elfb200_mcts_tree_usage": (ctypes.c_int, [vp, vp, vp]),
+    "elfb200_mcts_reset_dev": (ctypes.c_int, [vp, vp]),
+    "elfb200_mcts_begin_move_dev": (ctypes.c_int, [vp, vp, vp]),
+    "elfb200_mcts_select_dev": (ctypes.c_int, [vp, vp, ctypes.c_int, ctypes.c_int]),
+    "elfb200_mcts_expand_backup_dev": (ctypes.c_int, [vp, vp, vp]),
+    "elfb200_mcts_results_dev": (ctypes.c_int, [vp, vp, vp, vp, vp, vp]),
+    "elfb200_mcts_choose_dev": (ctypes.c_int, [vp, ctypes.c_int, ctypes.c_float, vp, vp, vp, vp]),
+    "elfb200_mcts_advance_dev": (ctypes.c_int, [vp, vp]),
 }
 
 

@@ -236,6 +236,120 @@ class MctsBatch(RefStreamSearch):
         ev[2].record(s_src)
         cur.wait_event(ev[2])
 
+    # -- search without the host: the device forms (elfb200_mcts_*_dev) -----------------------------------------
+    def _check_dev(self, t, dtypes, shape, name):
+        if t.device != self.device or t.dtype not in dtypes or tuple(t.shape) != shape or not t.is_contiguous():
+            raise ValueError(f"{name} must be a contiguous {'/'.join(map(str, dtypes))} tensor of shape {shape} on "
+                             f"{self.device}")
+
+    def _mask_dev(self, mask, name):
+        if mask is None:
+            return None
+        torch = self._torch
+        self._check_dev(mask, (torch.uint8, torch.bool), (self.gb.num_games,), name)
+        return mask.view(torch.uint8).data_ptr()
+
+    def _dev_call(self, call):
+        """``call`` on the context stream, ordered after the caller's current stream and before its next work:
+        events only, no host synchronisation (as ``GoEnv`` orders its calls)"""
+        cuda = self.device.type == "cuda"
+        if cuda:
+            if getattr(self, "_dev_ev", None) is None:
+                self._dev_ev = [self._torch.cuda.Event(), self._torch.cuda.Event()]
+            cur = self._torch.cuda.current_stream(self.device)
+            self._dev_ev[0].record(cur)
+            self._stream.wait_event(self._dev_ev[0])
+        call()
+        if cuda:
+            self._dev_ev[1].record(self._stream)
+            cur.wait_event(self._dev_ev[1])
+
+    def _dev_out(self):
+        """the fixed output tensors of choose_dev / results_dev, allocated on first use"""
+        if getattr(self, "_dev_tables", None) is None:
+            torch, G, P1, d = self._torch, self.gb.num_games, self.gb.num_actions, self.device
+            i32, f32 = torch.int32, torch.float32
+            self._dev_tables = {
+                "actions": torch.zeros(G, dtype=i32, device=d), "values": torch.zeros(G, dtype=f32, device=d),
+                "best_action": torch.zeros(G, dtype=i32, device=d), "visits": torch.zeros((G, P1), dtype=i32, device=d),
+                "root_value": torch.zeros(G, dtype=f32, device=d), "best_q": torch.zeros(G, dtype=f32, device=d),
+                "total_visits": torch.zeros(G, dtype=i32, device=d)}
+        return self._dev_tables
+
+    def search_dev(self, actor, move, active=None):
+        """One whole move (``begin_move`` and ``waves_per_move`` waves) without the host: nothing is read back and
+        the host never waits, so the call can be captured in a CUDA graph -- a graph must hold whole moves, because
+        each wave's D4 codes are keyed by the wave index, which the host passes by value.
+
+        ``move``: int64 [1] tensor on this handle's device, the move index that keys the root noise (the host form
+        keys it by a host counter, which would be frozen in a graph: advance the tensor, e.g. ``move.add_(1)``,
+        so that every replay draws fresh noise).  ``active``: uint8 / bool [G] tensor, or None (all games).
+
+        ``actor(batch) -> {"pi", "V"}`` is called every wave on the full ``max_leaves`` feature view
+        (``batch[self.feat_key]``); rows past the device-side leaf count are stale and their replies are ignored.
+        Inside a capture the actor must itself be capturable: no host synchronisation and no graph of its own.
+        ``FusedActor(cuda_graph=True)`` replays its own graph, so it can only be used uncaptured; plain
+        ``PolicyValueNet``, ``Actor`` and ``FusedActor(cuda_graph=False)`` should be capturable, which is not
+        verified here (``scripts/search_graph_bench.py`` captures the actor it uses).
+
+        Ordering with the caller's current stream uses events only.  There is no ``strict_root`` check: a root
+        that does not match its board is counted in ``errors()[0]`` and rebuilt.  Host-side counters do not see
+        work replayed from a graph (``timings``); the device counters (``stats``, ``errors``, ``eval_count``) do."""
+        torch = self._torch
+        self._check_dev(move, (torch.int64,), (1,), "move")
+        act = self._mask_dev(active, "active")
+        cuda = self.device.type == "cuda"
+        L, m = self._lib, self._m
+        self._dev_call(lambda: _l.check(L, L.elfb200_mcts_begin_move_dev(m, act, move.data_ptr())))
+        for _ in range(self.waves_per_move):
+            self._dev_call(lambda: _l.check(L, L.elfb200_mcts_select_dev(m, self.feat.data_ptr(), self._fmt, self.cpad)))
+            with torch.no_grad():
+                reply = actor({self.feat_key: self.feat})
+                pi = reply["pi"].to(torch.float32).contiguous()
+                v = reply["V"].to(torch.float32).reshape(-1).contiguous()
+            if pi.shape[0] < self.max_leaves or v.shape[0] < self.max_leaves or pi.device != self.device:
+                raise ValueError(f"the actor must answer all {self.max_leaves} rows on {self.device}")
+            self._dev_call(lambda: _l.check(L, L.elfb200_mcts_expand_backup_dev(m, pi.data_ptr(), v.data_ptr())))
+            # the reply is read on the context stream, which the caching allocator knows nothing about
+            self._keep = (pi, v) if cuda else None
+
+    def choose_dev(self, policy_distri_cutoff, resign_thres, seed, never_resign=None):
+        """``choose`` with the seed read from ``seed`` (int64 [1] tensor on this handle's device) when the kernel
+        runs, so a graph replay draws with the seed the tensor then holds; ``never_resign``: uint8 / bool [G]
+        tensor or None.  Returns this handle's fixed (actions int32 [G], values float32 [G]) tensors: their
+        addresses stay the same across calls, and each call overwrites them."""
+        torch = self._torch
+        self._check_dev(seed, (torch.int64,), (1,), "seed")
+        nr = self._mask_dev(never_resign, "never_resign")
+        out = self._dev_out()
+        a, v = out["actions"], out["values"]
+        L, m = self._lib, self._m
+        self._dev_call(lambda: _l.check(L, L.elfb200_mcts_choose_dev(
+            m, int(policy_distri_cutoff), float(resign_thres), nr, seed.data_ptr(), a.data_ptr(), v.data_ptr())))
+        return a, v
+
+    def results_dev(self):
+        """``results`` into this handle's fixed tensors on its device (the same dict of tensors every call)"""
+        o = self._dev_out()
+        r = {k: o[k] for k in ("best_action", "visits", "root_value", "best_q", "total_visits")}
+        L, m = self._lib, self._m
+        self._dev_call(lambda: _l.check(L, L.elfb200_mcts_results_dev(
+            m, *(r[k].data_ptr() for k in ("best_action", "visits", "root_value", "best_q", "total_visits")))))
+        return r
+
+    def advance_dev(self, actions):
+        """``advance`` from an int32 [G] tensor on this handle's device (< 0: the game's tree is untouched)"""
+        torch = self._torch
+        self._check_dev(actions, (torch.int32,), (self.gb.num_games,), "actions")
+        L, m = self._lib, self._m
+        self._dev_call(lambda: _l.check(L, L.elfb200_mcts_advance_dev(m, actions.data_ptr())))
+
+    def reset_dev(self, mask=None):
+        """``reset`` for the games where the uint8 / bool [G] tensor ``mask`` is set (None: every game)"""
+        mp = self._mask_dev(mask, "mask")
+        L, m = self._lib, self._m
+        self._dev_call(lambda: _l.check(L, L.elfb200_mcts_reset_dev(m, mp)))
+
     def tree_usage(self):
         """(nodes, edges) int32 [G] each: in-use nodes and stored edges of the visited nodes of every game's
         tree, the records ``gather`` copies for the game"""

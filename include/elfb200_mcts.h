@@ -179,6 +179,54 @@ int elfb200_mcts_gather_dev(elfb200_mcts* dst, const elfb200_mcts* src, const in
  * elfb200_mcts_gather copies for the game. */
 int elfb200_mcts_tree_usage(elfb200_mcts* m, int32_t* nodes_host, int32_t* edges_host);
 
+/* ---- Search without the host: the device forms ------------------------------------------------------------
+ * Every pointer is device memory.  Each call only enqueues work on the context stream: no host synchronisation,
+ * no host<->device copy, no event record, no allocation, so the calls can be captured in a CUDA graph from their
+ * first call.  They launch the kernels of their host forms, and compute what those compute:
+ *     elfb200_mcts_reset_dev(m, mask)                    elfb200_mcts_reset
+ *     elfb200_mcts_begin_move_dev(m, active, move)       elfb200_mcts_begin_move
+ *     elfb200_mcts_select_dev(m, feat, format, cpad)     elfb200_mcts_select_ex(..., n_leaves = NULL)
+ *     elfb200_mcts_expand_backup_dev(m, pi, value)       elfb200_mcts_expand_backup
+ *     elfb200_mcts_results_dev(m, ...)                   elfb200_mcts_results
+ *     elfb200_mcts_choose_dev(m, ..., seed, ...)         elfb200_mcts_choose
+ *     elfb200_mcts_advance_dev(m, actions)               elfb200_mcts_advance
+ * The random draws that the host forms key by a value passed by value are keyed by device memory here, so a
+ * replayed graph draws what the caller's counters hold at replay time: the root noise by (seed, (uint32)*move_dev),
+ * as begin_move keys it by its host move counter (which the device form neither reads nor advances); the move
+ * choice by *seed_dev, bit for bit the host form's key with that seed.
+ * A whole move is begin_move_dev, then elfb200_mcts_waves_per_move x (select_dev, the network on all
+ * elfb200_mcts_max_leaves rows, expand_backup_dev).  The D4 code of each leaf is keyed by the wave index, which the
+ * host passes by value and begin_move_dev sets back to 0: a graph must therefore capture whole moves.
+ * Host-side counters do not see work replayed from a graph: elfb200_mcts_timings never counts the device forms, and
+ * elfb200_mcts_eval_count in synchronous mode counts host-form waves only (after a select_dev it reads the device
+ * total, as in the asynchronous mode).  The device counters (elfb200_mcts_stats, elfb200_mcts_errors) see every
+ * wave.  A root that does not match its board is counted in elfb200_mcts_errors [0] and rebuilt.
+ * Refused with nothing enqueued: NULL handle (ELFB200_ERR_ARG); any device form while a reference D4 stream is set
+ * (ELFB200_ERR_STATE: elfb200_mcts_set_d4_stream is fed from the host every move). */
+/* reset for the games with mask_dev[g] != 0 (uint8[G], NULL = all games). */
+int elfb200_mcts_reset_dev(elfb200_mcts* m, const uint8_t* mask_dev);
+/* active_dev uint8[G] (NULL = all active) copied device to device, then begin_move; move_dev int64[1] keys the
+ * root noise and may be NULL only with root_epsilon == 0 (ELFB200_ERR_ARG).  Sets the wave index back to 0.
+ * ELFB200_ERR_STATE while a wave is open. */
+int elfb200_mcts_begin_move_dev(elfb200_mcts* m, const uint8_t* active_dev, const int64_t* move_dev);
+/* The asynchronous select, in any format elfb200_mcts_select_ex accepts; the leaf count stays on the device and the
+ * feature grid covers all G*B slots.  ELFB200_ERR_ARG for a NULL feat_dev or a bad format, ELFB200_ERR_STATE while
+ * a wave is open. */
+int elfb200_mcts_select_dev(elfb200_mcts* m, void* feat_dev, int format, int cpad);
+/* Expansion and backup with elfb200_mcts_max_leaves reply rows (rows past the device-side count are ignored).
+ * ELFB200_ERR_ARG for NULL pi / value, ELFB200_ERR_STATE when no wave is open. */
+int elfb200_mcts_expand_backup_dev(elfb200_mcts* m, const float* pi_dev, const float* value_dev);
+/* The tables of elfb200_mcts_results into device arrays, each may be NULL. */
+int elfb200_mcts_results_dev(elfb200_mcts* m, int32_t* best_action_dev, int32_t* visits_dev, float* root_value_dev,
+                             float* best_q_dev, int32_t* total_visits_dev);
+/* choose with the seed read from seed_dev (int64[1]); never_resign_dev uint8[G] may be NULL, values_dev may be NULL.
+ * ELFB200_ERR_ARG for NULL seed_dev or actions_dev. */
+int elfb200_mcts_choose_dev(elfb200_mcts* m, int policy_distri_cutoff, float resign_thres,
+                            const uint8_t* never_resign_dev, const int64_t* seed_dev, int32_t* actions_dev,
+                            float* values_dev);
+/* advance from a device array int32[G] (actions[g] < 0: untouched).  ELFB200_ERR_ARG for NULL actions_dev. */
+int elfb200_mcts_advance_dev(elfb200_mcts* m, const int32_t* actions_dev);
+
 #ifdef __cplusplus
 }
 #endif
